@@ -1,7 +1,7 @@
-"""adanet_b200: a B200-native AdaNet candidate-training engine behind the
+"""adanet_b200: an H100-native AdaNet candidate-training engine behind the
 tensorflow/adanet API surface (adanet/__init__.py:21-59 of the reference).
 
-The per-iteration hot path runs as hand-written sm_100a CUDA kernels
+The per-iteration hot path runs as hand-written sm_90a CUDA kernels
 (adanet_b200/csrc, C ABI in include/adanet_b200.h); this package is the
 host-side mirror of the reference's plugin interface over it.  Importing the
 package needs neither a GPU nor the built extension; any compute entry point

@@ -2,7 +2,7 @@
 
 No torch types cross this boundary: tensors are passed as ``data_ptr()``
 integers and the CUDA stream as its raw handle.  The shared library is built
-in-tree by ``__graft_entry__.build()`` (nvcc, sm_100a); if it is missing the
+in-tree by ``__graft_entry__.build()`` (nvcc, sm_90a); if it is missing the
 import of any compute entry point fails loudly -- there is no CPU fallback.
 """
 

@@ -6,7 +6,7 @@ The reference builds a TF1 graph per AdaNet iteration
 candidate ensemble's train op in one `session.run` per step through hooks
 (adanet/core/iteration.py:150-205,961-996).  Here an :class:`IterationPlan`
 owns, for the candidates placed on this GPU, all parameters, activations,
-gradients and bookkeeping in HBM and enqueues the hand-written sm_100a kernels
+gradients and bookkeeping in HBM and enqueues the hand-written sm_90a (H100) kernels
 of ``adanet_b200/csrc`` through the C ABI (include/adanet_b200.h):
 
   frozen members  -> adn_dense_fwd (forward-only replay, shared by all candidates)
@@ -14,7 +14,7 @@ of ``adanet_b200/csrc`` through the C ABI (include/adanet_b200.h):
   candidate head  -> adn_ensemble_head (+ adn_opt_step on the mixture weights)
   EMA / steps     -> adn_ema_update / adn_record_scalars / adn_counter_add
 
-Dense layers run on the plane-native tcgen05 pipeline (csrc/planes.cu): the
+Dense layers run on the plane-native tensor-core pipeline (csrc/planes.cu): the
 minibatch is split into hi/lo planes (fp16 pairs by default, TF32 pairs as the
 fallback: csrc/plane_fmt.cuh) once per step, every hidden activation and
 back-propagated gradient stays in plane format between GEMMs
@@ -68,7 +68,7 @@ def _stream_ptr(stream: Optional[torch.cuda.Stream] = None) -> int:
 
 def _require_cuda():
   if not torch.cuda.is_available():
-    raise _lib.AdnError("adanet_b200 engine needs a CUDA device (sm_100a); there is no CPU fallback.")
+    raise _lib.AdnError("adanet_b200 engine needs a CUDA device (sm_90a); there is no CPU fallback.")
   lib = _lib.load()
   _lib.check(lib.adn_init(), "adn_init")
   return lib

@@ -1,4 +1,4 @@
-// C-ABI glue: error state, queries, dense path dispatch (SIMT fp32 vs tcgen05 split planes).
+// C-ABI glue: error state, queries, dense path dispatch (SIMT fp32 vs tensor-core split planes).
 #include <stdarg.h>
 #include <stdlib.h>
 #include <string.h>
@@ -32,7 +32,7 @@ int sm_count() {
   if (cudaGetDevice(&dev) != cudaSuccess ||
       cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) {
     (void)cudaGetLastError();
-    n = 148;  // B200
+    n = 132;  // H100 SXM
   }
   g_sm_count.store(n);
   return n;

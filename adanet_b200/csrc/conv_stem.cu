@@ -1,5 +1,5 @@
 // K6: the SimpleCNN stem -- Conv2D(F, 3x3, "same") + bias + ReLU -> MaxPool2D(2, 2) -> Flatten -- fused into one
-// forward kernel that writes the pooled features straight into the split-plane format the tcgen05 dense
+// forward kernel that writes the pooled features straight into the split-plane format the tensor-core dense
 // pipeline consumes (planes.cu), and one backward kernel for the kernel / bias gradients.
 //
 // Replaces the Keras layers of SimpleCNNBuilder.build_subnetwork in
@@ -7,7 +7,7 @@
 //   x = Conv2D(filters=16, kernel_size=3, padding="same", activation="relu")(images)
 //   x = MaxPool2D(pool_size=2, strides=2)(x);  x = Flatten()(x)            [TF/Keras, NHWC, HWIO kernel]
 //
-// Why SIMT fp32 and not tcgen05: the contraction is K = 9*Cin = 27 by N = F = 16 -- per example 0.44 MFMA against
+// Why SIMT fp32 and not the tensor cores: the contraction is K = 9*Cin = 27 by N = F = 16 -- per example 0.44 MFMA against
 // 12 KB of image read and ~37 KB of planes written, i.e. the kernel sits between the FP32-FMA rate and HBM, and
 // an implicit-GEMM tile (K padded to 32, N=16) would leave the tensor pipe >90 % idle while adding an im2col
 // stage.  Exact fp32 FMAs also keep the conv bit-comparable with the fp32 cross-check.
@@ -39,14 +39,14 @@ int fwd(const float* images, const float* kernel, const float* bias, void* out_p
 
 namespace conv {
 
-// ADN_CONV_PATH=simt forces the exact-fp32 SIMT forward (cross-check); default: tcgen05 implicit GEMM where supported
+// ADN_CONV_PATH=simt forces the exact-fp32 SIMT forward (cross-check); default: the wgmma implicit GEMM (conv_stem_tc.cu) where supported
 static bool use_tc() {      // read per call (host side, cheap): tests switch it at run time
   const char* e = getenv("ADN_CONV_PATH");
   return !(e && (e[0] == 's' || e[0] == 'S'));
 }
 
-// The tcgen05 backward (conv_stem_tc.cu) is correct but, with its serial build -> MMA -> drain per warpgroup, slower
-// than the SIMT gather (204 vs 136 us at B=4096, profiles/r1h_conv_tc_*.txt): opt-in with ADN_CONV_BWD_PATH=tcgen05.
+// The tensor-core backward (conv_stem_tc.cu) serialises build -> MMA -> drain per warpgroup; the SIMT gather stays the
+// default and the tensor-core variant is opt-in with ADN_CONV_BWD_PATH=tcgen05 (the value keeps its historical name).
 static bool use_tc_bwd() {
   const char* e = getenv("ADN_CONV_BWD_PATH");
   return e && (e[0] == 't' || e[0] == 'T');

@@ -1,4 +1,4 @@
-// K6b: the SimpleCNN stem forward as a tcgen05 implicit GEMM (same contract as conv_stem_fwd_kernel in
+// K6b: the SimpleCNN stem forward as a wgmma implicit GEMM (same contract as conv_stem_fwd_kernel in
 // conv_stem.cu, which stays as the exact-fp32 cross-check path: ADN_CONV_PATH=simt).
 //
 // Formulation: rows = POOLED pixels, not conv positions.  For one pooled pixel the four conv positions of its 2x2
@@ -6,21 +6,22 @@
 //     acc[p][(pos, f)] = sum_k A[p][k] * W'[k][(pos, f)],   k = (i, j, c) over the 4x4xCin patch (K = 16*Cin),
 //     W'[(i,j,c)][(dy,dx,f)] = w[i-dy][j-dx][c][f]  (zero outside the 3x3 support),   N = 4*F,
 // is a [128 x K] x [K x N] GEMM per 128 pooled pixels whose accumulator row holds exactly what the epilogue thread
-// of the SIMT kernel holds in registers: 4 positions x F filters of its own pooled pixel.  Bias, ReLU, the 2x2
-// max, the arg-max, the TF32 hi/lo split and the plane stores therefore happen in one thread per pooled pixel,
-// straight out of TMEM, with no cross-lane traffic.  The price is 1.78x the minimal MACs (zeros in W'), irrelevant
-// at 3 x 6 tcgen05.mma (M128 N64 K8) per tile.
+// of the SIMT kernel holds in registers: 4 positions x F filters of its own pooled pixel.  A thread of the wgmma
+// accumulator layout holds the 4 positions of the same filters, so bias, ReLU, the 2x2 max and the arg-max stay in
+// the thread; sign-bit and arg-max words are OR-ed over the 4 threads of a row.  The price is 1.78x the minimal MACs
+// (zeros in W'), irrelevant at 3 x 6 wgmma (M64 N64 K8) per 64 pooled pixels.
 //
-// fp32 accuracy: 3xTF32 (a_hi b_hi + a_lo b_hi + a_hi b_lo), K <= 48, one TMEM accumulator.
+// fp32 accuracy: 3xTF32 (a_hi b_hi + a_lo b_hi + a_hi b_lo), K <= 48, one accumulator.
 //
 // Per CTA (256 threads = 2 warpgroups, 1 CTA per SM): the image is staged zero-padded in shared memory with
 // cp.async (double buffered); each warpgroup takes a tile of 128 pooled pixels: every thread gathers its own A row
 // from the staged image (LDS.64), splits it and writes hi / lo in the canonical K-major SWIZZLE_128B layout
-// (16-byte chunk index XOR row%8 -- what TMA would have produced), fence.proxy.async, one elected thread issues
-// the MMAs and commits to the warpgroup's mbarrier, then all 128 threads read their accumulator row with
-// tcgen05.ld (warp w reads TMEM lanes 32(w%4)..) and run the epilogue.  W' (hi / lo, K-major) is built once per CTA.
+// (16-byte chunk index XOR row%8 -- what TMA would have produced), fence.proxy.async, then the warpgroup issues
+// the MMAs of each 64-row half and runs the epilogue on the registers they return.  W' (hi / lo, K-major) is built
+// once per CTA.
 #include "common.cuh"
 #include "plane_fmt.cuh"
+#include "wgmma.cuh"
 
 namespace adn {
 namespace convtc {
@@ -38,78 +39,20 @@ __device__ __forceinline__ void cp_async4(void* smem, const void* gmem) {
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-// Bounded spin: a broken pipeline traps (CUDA error) instead of hanging the GPU box.
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t ok = 0;
-  long long t0 = 0;
-  for (uint32_t it = 0;; ++it) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(bar), "r"(parity)
-        : "memory");
-    if (ok) return;
-    if ((it & 1023u) == 1023u) {
-      long long now = clock64();
-      if (t0 == 0) t0 = now;
-      else if (now - t0 > 4000000000LL) __trap();
-    }
-  }
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void wg_barrier(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
-// K-major SWIZZLE_128B smem descriptor (cute::UMMA::SmemDescriptor): start >> 4 | LBO(unused)=1 << 16 |
-// SBO = 1024 B >> 4 at [32,46) | version 1 at [46,48) | layout type 2 at [61,64)
-__device__ __forceinline__ uint32_t desc_lo(uint32_t addr) { return ((addr & 0x3FFFFu) >> 4) | (1u << 16); }
-__device__ __forceinline__ uint32_t desc_hi() { return (uint32_t)(1024 >> 4) | (1u << 14) | (2u << 29); }
-// kind::tf32 instruction descriptor: D=f32, A=B=tf32, both K-major, N>>3 at [17,23), M>>4 at [24,29)
-__device__ __forceinline__ uint32_t make_idesc(int m, int n) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
-}
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint32_t da, uint32_t db, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-      "mov.b64 da, {%1, %3};\n\t"
-      "mov.b64 db, {%2, %3};\n\t"
-      "setp.ne.b32 p, %5, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], da, db, %4, p;\n\t}"
-      ::"r"(tmem_d), "r"(da), "r"(db), "r"(desc_hi()), "r"(idesc), "r"(accum)
-      : "memory");
-}
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t.reg .pred P;\n\t"
-      "elect.sync _|P, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, P;\n\t}"
-      : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&r)[16]) {
-  uint32_t u[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(u[0]), "=r"(u[1]), "=r"(u[2]), "=r"(u[3]), "=r"(u[4]), "=r"(u[5]), "=r"(u[6]), "=r"(u[7]),
-        "=r"(u[8]), "=r"(u[9]), "=r"(u[10]), "=r"(u[11]), "=r"(u[12]), "=r"(u[13]), "=r"(u[14]), "=r"(u[15])
-      : "r"(taddr));
-#pragma unroll
-  for (int i = 0; i < 16; ++i) r[i] = __uint_as_float(u[i]);
-}
 // byte offset of element (row, k) inside one k-block tile ([rows][32 floats], SWIZZLE_128B)
 __device__ __forceinline__ uint32_t sw128(int row, int k) {
   return (uint32_t)((row >> 3) * 1024 + (row & 7) * 128 + ((((k >> 2) ^ (row & 7)) & 7) << 4) + ((k & 3) << 2));
+}
+// D (+)= A B over one K step of 8, tf32, both operands K-major SWIZZLE_128B tiles in shared memory
+template <int N>
+__device__ __forceinline__ void mma_tf32(float (&d)[N / 2], uint32_t a_addr, uint32_t b_addr, uint32_t scale_d) {
+  const uint64_t da = wg::desc_sw128(a_addr), db = wg::desc_sw128(b_addr);
+  if constexpr (N == 16) wg::mma_tf32_n16(d, da, db, scale_d);
+  else if constexpr (N == 48) wg::mma_tf32_n48(d, da, db, scale_d);
+  else if constexpr (N == 64) wg::mma_tf32_n64(d, da, db, scale_d);
+  else wg::mma_tf32_n128(d, da, db, scale_d);
 }
 
 template <int CIN>
@@ -124,33 +67,16 @@ __device__ __forceinline__ void stage_image(float* s_img, const float* img, int 
   }
 }
 
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float (&r)[8]) {
-  uint32_t u[8];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-      : "=r"(u[0]), "=r"(u[1]), "=r"(u[2]), "=r"(u[3]), "=r"(u[4]), "=r"(u[5]), "=r"(u[6]), "=r"(u[7])
-      : "r"(taddr));
-#pragma unroll
-  for (int i = 0; i < 8; ++i) r[i] = __uint_as_float(u[i]);
-}
-
-static constexpr int FWD_THREADS = 512;
 // staged-image ring depth of the forward: 4 where shared memory allows (F = 16), else 2
 __host__ __device__ constexpr int fwd_image_buffers(int f) { return f == 16 ? 4 : 2; }
 
-// Forward, warp specialised.  512 threads = 4 warpgroups over two pipeline slots s = 0, 1 (a slot = one A tile
-// buffer + two TMEM accumulators):
-//   warpgroup s     (builders of slot s): stage images (with the other builders), gather / split / swizzle the A
-//                   rows of a tile, issue the MMAs of the tile (one elected thread) and commit to acc_full[s][a];
-//   warpgroup 2 + s (epilogue of slot s): wait acc_full[s][a], tcgen05.ld the accumulator, release it (acc_free), then
-//                   bias / ReLU / pool / split / store while the builders are already on the next tile.
-// Shared memory (from a 1024-aligned base): W' hi|lo [2][KB][N][128 B]; A per slot hi|lo [2][KB][16 KB]; two padded
-// images; bias; mbarriers acc_full[2][2], acc_free[2][2]; TMEM slot.
+// Forward.  256 threads = 2 warpgroups; warpgroup s takes the tiles s, s + 2, ... of every image: gather / split /
+// swizzle the A rows of the tile, then per 64-row half issue the 3 x K/8 MMAs, wait, and run bias / ReLU / pool /
+// split / store on the returned accumulators.
+// Shared memory (from a 1024-aligned base): W' hi|lo [2][KB][N][128 B]; A per warpgroup hi|lo [2][KB][16 KB]; the
+// ring of padded images; bias.
 template <int CIN, int F>
-__global__ void __launch_bounds__(FWD_THREADS, 1)
+__global__ void __launch_bounds__(THREADS, 1)
 conv_stem_tc_fwd_kernel(const float* __restrict__ images, const float* __restrict__ kernel, const float* __restrict__ bias,
                         const pl::PlaneView pv, unsigned int* ovf,
                         uint32_t* __restrict__ argmax, int64_t B, int H, int W) {
@@ -158,24 +84,21 @@ conv_stem_tc_fwd_kernel(const float* __restrict__ images, const float* __restric
   constexpr int KB = (K + 31) / 32;        // k-blocks of 32 floats (128 B swizzle atoms)
   constexpr int N = 4 * F;                 // (pool position, filter)
   constexpr int NB = N * 128;              // bytes of one k-block of W'
-  constexpr int TMEM_COLS = 4 * N < 32 ? 32 : 4 * N;   // 2 slots x 2 accumulators of N columns (N = 64 / 128 -> 256 / 512)
   constexpr int NBUF = fwd_image_buffers(F);           // ring of staged images: the fetch of image i+NBUF-1 runs under image i
+  constexpr int FJ = F / 8;                // 8-column fragment groups per pool position
   extern __shared__ __align__(16) uint8_t smem_raw[];
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* s_w = base;                                  // [2 planes][KB][N][128 B]
-  uint8_t* s_a = s_w + 2 * KB * NB;                     // [2 slots][2 planes][KB][16 KB]
+  uint8_t* s_a = s_w + 2 * KB * NB;                     // [2 warpgroups][2 planes][KB][16 KB]
   const int pimg = (H + 2) * (W + 2) * CIN;
   float* s_img0 = reinterpret_cast<float*>(s_a + 2 * 2 * KB * TILE_BYTES);
   float* s_b = s_img0 + NBUF * pimg;
-  uint64_t* s_bar = reinterpret_cast<uint64_t*>(s_b + F);      // [0,4) acc_full[slot][acc], [4,8) acc_free[slot][acc]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(s_bar + 8);
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int wgi = tid >> 7, r = tid & 127;
-  const int slot = wgi & 1;
-  const bool builder = wgi < 2;
-  // ---- once per CTA: W' (hi / lo, K-major swizzled), bias, zero borders of the image buffers, barriers, TMEM ----
-  for (int idx = tid; idx < N * K; idx += FWD_THREADS) {
+  const int tid = threadIdx.x, lane = tid & 31;
+  const int slot = tid >> 7, r = tid & 127, wq = (tid >> 5) & 3;
+  const int gid = lane >> 2, tq = lane & 3;
+  // ---- once per CTA: W' (hi / lo, K-major swizzled), bias, zero borders of the image buffers ----
+  for (int idx = tid; idx < N * K; idx += THREADS) {
     const int n = idx / K, k = idx - n * K;
     const int pos = n / F, f = n - pos * F;
     const int c = k % CIN, ij = k / CIN;
@@ -186,67 +109,43 @@ conv_stem_tc_fwd_kernel(const float* __restrict__ images, const float* __restric
     *reinterpret_cast<float*>(s_w + off) = h;
     *reinterpret_cast<float*>(s_w + KB * NB + off) = rna_tf32(v - h);
   }
-  for (int i = tid; i < F; i += FWD_THREADS) s_b[i] = bias[i];
-  for (int i = tid; i < NBUF * pimg; i += FWD_THREADS) s_img0[i] = 0.f;
-  if (warp == 0) {
-    if (lane == 0) {
-      for (int i = 0; i < 4; ++i) mbar_init(smem_u32(&s_bar[i]), 1);
-      for (int i = 4; i < 8; ++i) mbar_init(smem_u32(&s_bar[i]), 128);
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "r"((uint32_t)TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
+  for (int i = tid; i < F; i += THREADS) s_b[i] = bias[i];
+  for (int i = tid; i < NBUF * pimg; i += THREADS) s_img0[i] = 0.f;
   fence_async_smem();          // W' was written through the generic proxy, the MMAs read it through the async proxy
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // one full / free barrier pair PER ACCUMULATOR: a full barrier can then never run two phases ahead of the epilogue
-  // (the next commit to the same accumulator needs the epilogue's release of the previous one)
-  const uint32_t acc_full0 = smem_u32(&s_bar[2 * slot]);
-  const uint32_t acc_free0 = smem_u32(&s_bar[4 + 2 * slot]);
 
   const int PH = H / 2, PW = W / 2, P = PH * PW;
   const int tiles = (P + 127) / 128;
   const int prow = (W + 2) * CIN;
   const int64_t img_elems = (int64_t)H * W * CIN;
-
-  if (builder) {
-    // =========================== builders: images -> A tiles -> MMAs ===========================
-    const uint32_t idesc = make_idesc(128, N);
-    const uint32_t w_addr = smem_u32(s_w);
-    uint8_t* a_hi = s_a + slot * (2 * KB * TILE_BYTES);
-    uint8_t* a_lo = a_hi + KB * TILE_BYTES;
-    const uint32_t a_addr = smem_u32(a_hi);
-    const int btid = tid;                      // 0..255 among the builders
-    uint32_t n_tiles = 0;                      // tiles this slot has issued so far
-    int64_t b = blockIdx.x;
-    for (int i = 0; i < NBUF - 1; ++i) {       // prologue: the first NBUF-1 images of this CTA
-      const int64_t bi = b + (int64_t)i * gridDim.x;
-      if (bi < B) stage_image<CIN>(s_img0 + i * pimg, images + bi * img_elems, H, W, btid, 256);
-      cp_async_commit();
-    }
-    int buf = 0;
-    for (; b < B; b += gridDim.x, buf = (buf + 1 == NBUF) ? 0 : buf + 1) {
-      cp_async_wait<NBUF - 2>();                       // this thread's copies of image b have landed
-      asm volatile("bar.sync 3, 256;" ::: "memory");   // image b is visible to both builder warpgroups; image b-1 is no longer read
-      const int64_t nb = b + (int64_t)(NBUF - 1) * gridDim.x;
-      const int pbuf = (buf == 0) ? NBUF - 1 : buf - 1;    // the buffer image b-1 used
-      if (nb < B) stage_image<CIN>(s_img0 + pbuf * pimg, images + nb * img_elems, H, W, btid, 256);
-      cp_async_commit();
-      const float* s_img = s_img0 + buf * pimg;
-      for (int tile = slot; tile < tiles; tile += 2, ++n_tiles) {
+  const int64_t words_per_row = (int64_t)P * F / 16;
+  const uint32_t w_addr = smem_u32(s_w);
+  uint8_t* a_hi = s_a + slot * (2 * KB * TILE_BYTES);
+  uint8_t* a_lo = a_hi + KB * TILE_BYTES;
+  const uint32_t a_addr = smem_u32(a_hi);
+  int64_t b = blockIdx.x;
+  for (int i = 0; i < NBUF - 1; ++i) {       // prologue: the first NBUF-1 images of this CTA
+    const int64_t bi = b + (int64_t)i * gridDim.x;
+    if (bi < B) stage_image<CIN>(s_img0 + i * pimg, images + bi * img_elems, H, W, tid);
+    cp_async_commit();
+  }
+  int buf = 0;
+  for (; b < B; b += gridDim.x, buf = (buf + 1 == NBUF) ? 0 : buf + 1) {
+    cp_async_wait<NBUF - 2>();                       // this thread's copies of image b have landed
+    __syncthreads();                                 // image b is visible to both warpgroups; image b-1 is no longer read
+    const int64_t nb = b + (int64_t)(NBUF - 1) * gridDim.x;
+    const int pbuf = (buf == 0) ? NBUF - 1 : buf - 1;    // the buffer image b-1 used
+    if (nb < B) stage_image<CIN>(s_img0 + pbuf * pimg, images + nb * img_elems, H, W, tid);
+    cp_async_commit();
+    const float* s_img = s_img0 + buf * pimg;
+    for (int tile = slot; tile < tiles; tile += 2) {
+      {
         const int p = tile * 128 + r;
         const bool valid = p < P;
         const int py = valid ? p / PW : 0, px = valid ? p - py * PW : 0;
         const float* patch = s_img + (2 * py) * prow + (2 * px) * CIN;
         const uint32_t rowoff = (uint32_t)((r >> 3) * 1024 + (r & 7) * 128);
-        // the previous tile's MMAs must have finished reading this slot's A buffer
-        if (n_tiles > 0) mbar_wait(acc_full0 + 8 * ((n_tiles - 1) & 1u), ((n_tiles - 1) >> 1) & 1u);
+        wg_barrier(slot);                            // the previous tile's MMAs have finished reading this A buffer
 #pragma unroll
         for (int q = 0; q < K / 4; ++q) {
           const int i = (CIN == 3) ? q / 3 : q;
@@ -264,103 +163,80 @@ conv_stem_tc_fwd_kernel(const float* __restrict__ images, const float* __restric
         }
         fence_async_smem();
         wg_barrier(slot);
-        if ((warp & 3) == 0) {
-          if (elect_one()) {
-            const uint32_t accsel = n_tiles & 1u;
-            // the epilogue must have drained this accumulator (tile n_tiles - 2); a fresh barrier passes at parity 1
-            mbar_wait(acc_free0 + 8 * accsel, ((n_tiles >> 1) & 1u) ^ 1u);
-            tc_fence_after();
-            const uint32_t tmem_acc = tmem_base + (uint32_t)((slot * 2 + accsel) * N);
-            uint32_t accum = 0;
+      }
+#pragma unroll 1
+      for (int half = 0; half < 2; ++half) {
+        float d[N / 2];
 #pragma unroll
-            for (int prod = 0; prod < 3; ++prod) {       // a_hi b_hi, a_lo b_hi, a_hi b_lo
-              const uint32_t aa = a_addr + (prod == 1 ? KB * TILE_BYTES : 0);
-              const uint32_t ww = w_addr + (prod == 2 ? KB * NB : 0);
+        for (int i = 0; i < N / 2; ++i) d[i] = 0.f;
+        wg::fence_regs(d);
+        wg::fence();
 #pragma unroll
-              for (int ks = 0; ks < K / 8; ++ks) {
-                const uint32_t da = desc_lo(aa + (ks >> 2) * TILE_BYTES + (ks & 3) * 32);
-                const uint32_t db = desc_lo(ww + (ks >> 2) * NB + (ks & 3) * 32);
-                umma_tf32(tmem_acc, da, db, idesc, accum);
-                accum = 1;
+        for (int prod = 0; prod < 3; ++prod) {       // a_hi b_hi, a_lo b_hi, a_hi b_lo
+          const uint32_t aa = a_addr + (prod == 1 ? KB * TILE_BYTES : 0) + half * 8192;
+          const uint32_t ww = w_addr + (prod == 2 ? KB * NB : 0);
+#pragma unroll
+          for (int ks = 0; ks < K / 8; ++ks)
+            mma_tf32<N>(d, aa + (ks >> 2) * TILE_BYTES + (ks & 3) * 32, ww + (ks >> 2) * NB + (ks & 3) * 32,
+                        (prod == 0 && ks == 0) ? 0u : 1u);
+        }
+        wg::commit();
+        wg::wait<0>();
+        wg::fence_regs(d);
+        // ---- epilogue: rows 64 half + 16 wq + gid (+8); columns (pos, f) = 8 j + 2 tq + e, j = pos * FJ + fj ----
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) {
+          const int p = tile * 128 + 64 * half + 16 * wq + gid + 8 * rr;
+          const bool valid = p < P;
+#pragma unroll
+          for (int g16 = 0; g16 < F / 16; ++g16) {
+            uint32_t sign = 0u, arg = 0u;
+#pragma unroll
+            for (int h8 = 0; h8 < 2; ++h8) {
+              const int fj = 2 * g16 + h8;
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const int f = 8 * fj + 2 * tq + e;
+                const float bv = s_b[f];
+                float m = d[4 * fj + 2 * rr + e] + bv;
+                uint32_t a = 0u;
+#pragma unroll
+                for (int pos = 1; pos < 4; ++pos) {
+                  const float mp = d[4 * (pos * FJ + fj) + 2 * rr + e] + bv;
+                  if (mp > m) { m = mp; a = (uint32_t)pos; }
+                }
+                m = fmaxf(m, 0.f);
+                const int bit = f - 16 * g16;
+                sign |= (m > 0.f) ? (1u << bit) : 0u;
+                arg |= a << (2 * bit);
+                if (valid) pl::plane_store(pv, b, p * F + f, m, ovf);
               }
             }
-            umma_commit(acc_full0 + 8 * accsel);
-          }
-          __syncwarp();
-        }
-      }
-    }
-  } else {
-    // =========================== epilogue: accumulator -> pooled planes ===========================
-    const int64_t words_per_row = (int64_t)P * F / 16;
-    uint32_t n_tiles = 0;
-    for (int64_t b = blockIdx.x; b < B; b += gridDim.x) {
-      for (int tile = slot; tile < tiles; tile += 2, ++n_tiles) {
-        const int p = tile * 128 + r;
-        const bool valid = p < P;
-        const uint32_t accsel = n_tiles & 1u;
-        const uint32_t tmem_row = tmem_base + (uint32_t)((slot * 2 + accsel) * N) + ((uint32_t)((warp & 3) * 32) << 16);
-        mbar_wait(acc_full0 + 8 * accsel, (n_tiles >> 1) & 1u);
-        tc_fence_after();
-#pragma unroll 1
-        for (int f0 = 0; f0 < F; f0 += 16) {
-          uint32_t sign = 0u, arg = 0u;
-          const int64_t col0 = (int64_t)p * F + f0;
-#pragma unroll
-          for (int f8 = 0; f8 < 16; f8 += 8) {
-            float a0[8], a1[8], a2[8], a3[8];
-            tmem_ld8(tmem_row + (uint32_t)(0 * F + f0 + f8), a0);
-            tmem_ld8(tmem_row + (uint32_t)(1 * F + f0 + f8), a1);
-            tmem_ld8(tmem_row + (uint32_t)(2 * F + f0 + f8), a2);
-            tmem_ld8(tmem_row + (uint32_t)(3 * F + f0 + f8), a3);
-            tmem_ld_wait();
-            if (f0 + 16 >= F && f8 == 8) {       // last read of this accumulator: hand it back to the MMA issuer
-              tc_fence_before();
-              mbar_arrive(acc_free0 + 8 * accsel);
+            sign |= __shfl_xor_sync(0xffffffffu, sign, 1);
+            sign |= __shfl_xor_sync(0xffffffffu, sign, 2);
+            arg |= __shfl_xor_sync(0xffffffffu, arg, 1);
+            arg |= __shfl_xor_sync(0xffffffffu, arg, 2);
+            if (valid && tq == 0) {
+              const int64_t col0 = (int64_t)p * F + 16 * g16;
+              reinterpret_cast<uint16_t*>(pv.bits)[((col0 >> 5) * B + b) * 2 + ((col0 >> 4) & 1)] = (uint16_t)sign;
+              argmax[b * words_per_row + (col0 >> 4)] = arg;
             }
-            float outv[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const float bv = s_b[f0 + f8 + j];
-              float m = a0[j] + bv;
-              uint32_t a = 0u;
-              const float m1 = a1[j] + bv, m2 = a2[j] + bv, m3 = a3[j] + bv;
-              if (m1 > m) { m = m1; a = 1u; }
-              if (m2 > m) { m = m2; a = 2u; }
-              if (m3 > m) { m = m3; a = 3u; }
-              m = fmaxf(m, 0.f);
-              sign |= (m > 0.f) ? (1u << (f8 + j)) : 0u;
-              arg |= a << (2 * (f8 + j));
-              outv[j] = m;
-            }
-            if (valid) pl::plane_store8(pv, b, col0 + f8, outv, ovf);
-          }
-          if (valid) {
-            reinterpret_cast<uint16_t*>(pv.bits)[((col0 >> 5) * B + b) * 2 + ((col0 >> 4) & 1)] = (uint16_t)sign;
-            argmax[b * words_per_row + (col0 >> 4)] = arg;
           }
         }
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    __syncwarp();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)TMEM_COLS)
-                 : "memory");
   }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// Backward of the stem on tcgen05: with G'[p][(pos, f)] = g[p][f] * [argmax(p, f) == pos] (the pooled-feature
+// Backward of the stem on the tensor cores: with G'[p][(pos, f)] = g[p][f] * [argmax(p, f) == pos] (the pooled-feature
 // gradient routed to its arg-max position) the kernel gradient of the expanded weights is
 //     dW'[(pos, f)][k] = sum_p G'[p][(pos, f)] * A[p][k]
 // -- a GEMM whose reduction runs over pooled pixels, so both operands are staged TRANSPOSED (K-major in the pooled
-// index): M side = G'^T [4F rows (128 with zero rows)][64 px], N side = A^T [K rows][64 px], 3xTF32, 24 MMAs
-// (M128 N=K K8) per tile of 64 pooled pixels.  A warpgroup's 128 threads split a tile: threads 0-63 build A^T from the
-// staged image and later drain the accumulator, threads 64-127 fetch g / arg-max from global memory and build G'^T.
-// Two-level accumulation: TMEM holds one tile's sum, the drainers add it (RN) into registers; at the end
+// index): M side = G'^T [4F = 64 rows][64 px], N side = A^T [K rows][64 px], 3xTF32, 24 wgmma (M64 N=K K8) per tile
+// of 64 pooled pixels.  A warpgroup's 128 threads split the building of a tile: threads 0-63 build A^T from the
+// staged image, threads 64-127 fetch g / arg-max from global memory and build G'^T; all 128 issue the MMAs.
+// Two-level accumulation: the MMAs sum one tile, which is then added (RN) into a register accumulator; at the end
 // dK[ky,kx,c,f] = sum_pos dW'[(pos,f)][(ky+dy, kx+dx, c)] is folded in fixed order and written as this CTA's partial
 // (same format as the SIMT backward, reduced by conv_stem_reduce_kernel).
 template <int CIN, int F>
@@ -368,62 +244,38 @@ __global__ void __launch_bounds__(THREADS, 1)
 conv_stem_tc_bwd_kernel(const float* __restrict__ images, const uint32_t* __restrict__ argmax,
                         const float* __restrict__ dpooled, float* __restrict__ partials, int64_t B, int H, int W) {
   constexpr int K = 16 * CIN;              // patch size = GEMM N
-  static_assert(4 * F <= 64, "(pos, f) rows must fit TMEM lanes 0..63");
+  static_assert(4 * F == 64, "(pos, f) rows are the 64 rows of one wgmma");
   constexpr int PXT = 64;                  // pooled pixels per tile = GEMM K
-  constexpr int GB = 2 * TILE_BYTES;       // one plane of G'^T: 2 k-blocks of [128 rows][32 px]
+  constexpr int GB = 2 * TILE_BYTES;       // one plane of G'^T: 2 k-blocks of [128 rows][32 px] (rows 64.. unused)
   constexpr int AB = 2 * K * 128;          // one plane of A^T : 2 k-blocks of [K rows][32 px]
   constexpr int WGB = 2 * GB + 2 * AB;     // bytes per warpgroup
-  constexpr int TMEM_COLS = 128;           // two accumulators of K (<= 48) columns at column 0 and 64
   constexpr int K9 = 9 * CIN;
   extern __shared__ __align__(16) uint8_t smem_raw[];
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const int pimg = (H + 2) * (W + 2) * CIN;
   float* s_img0 = reinterpret_cast<float*>(base + 2 * WGB);
-  uint64_t* s_bar = reinterpret_cast<uint64_t*>(s_img0 + 2 * pimg);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(s_bar + 2);
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int wg = tid >> 7, r = tid & 127;
-  const int half = r >> 6, q = r & 63;     // half 0: A^T builder + drainer (TMEM lanes 0..63), half 1: G'^T builder
+  const int tid = threadIdx.x, lane = tid & 31;
+  const int wg = tid >> 7, r = tid & 127, wq = (tid >> 5) & 3;
+  const int gid = lane >> 2, tq = lane & 3;
+  const int half = r >> 6, q = r & 63;     // half 0: A^T builder, half 1: G'^T builder
   uint8_t* g_hi = base + wg * WGB;
   uint8_t* g_lo = g_hi + GB;
   uint8_t* at_hi = g_lo + GB;
   uint8_t* at_lo = at_hi + AB;
-  // zero everything once: rows MU..127 of G'^T stay zero for the whole kernel, image borders too
   for (int i = tid; i < (2 * WGB) / 16; i += THREADS) reinterpret_cast<float4*>(base)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
   for (int i = tid; i < 2 * pimg; i += THREADS) s_img0[i] = 0.f;
-  if (warp == 0) {
-    if (lane == 0) {
-      mbar_init(smem_u32(&s_bar[0]), 1);
-      mbar_init(smem_u32(&s_bar[1]), 1);
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "r"((uint32_t)TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  fence_async_smem();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_acc = tmem_base + (uint32_t)(wg * 64);
-  const uint32_t tmem_row = tmem_acc + ((uint32_t)((warp & 3) * 32) << 16);
-  const uint32_t idesc = make_idesc(128, K);
   const uint32_t g_addr = smem_u32(g_hi), at_addr = smem_u32(at_hi);
-  const uint32_t bar = smem_u32(&s_bar[wg]);
-  uint32_t phase = 0;
 
   const int PH = H / 2, PW = W / 2, P = PH * PW;
   const int tiles = (P + PXT - 1) / PXT;
   const int prow = (W + 2) * CIN;
   const int64_t img_elems = (int64_t)H * W * CIN;
   const int64_t cols = (int64_t)P * F;
-  float acc[K];                            // drainers: dW'[(pos, f) = q][k] summed over this CTA's tiles
+  float acc[K / 2];                        // dW' fragment: rows 16 wq + gid (+8), columns 8 j + 2 tq (+1)
 #pragma unroll
-  for (int k = 0; k < K; ++k) acc[k] = 0.f;
+  for (int k = 0; k < K / 2; ++k) acc[k] = 0.f;
   float accb[F];                           // G builders: sum of g over their pooled pixels, per filter
 #pragma unroll
   for (int f = 0; f < F; ++f) accb[f] = 0.f;
@@ -499,54 +351,42 @@ conv_stem_tc_bwd_kernel(const float* __restrict__ images, const uint32_t* __rest
         }
       }
       fence_async_smem();
-      tc_fence_before();
       wg_barrier(wg);
-      if ((warp & 3) == 0) {
-        if (elect_one()) {
-          tc_fence_after();
-          uint32_t accum = 0;
+      float d[K / 2];
 #pragma unroll
-          for (int prod = 0; prod < 3; ++prod) {       // g_hi a_hi, g_lo a_hi, g_hi a_lo
-            const uint32_t gg = g_addr + (prod == 1 ? GB : 0);
-            const uint32_t aa = at_addr + (prod == 2 ? AB : 0);
+      for (int k = 0; k < K / 2; ++k) d[k] = 0.f;
+      wg::fence_regs(d);
+      wg::fence();
 #pragma unroll
-            for (int ks = 0; ks < PXT / 8; ++ks) {
-              const uint32_t da = desc_lo(gg + (ks >> 2) * TILE_BYTES + (ks & 3) * 32);
-              const uint32_t db = desc_lo(aa + (ks >> 2) * (K * 128) + (ks & 3) * 32);
-              umma_tf32(tmem_acc, da, db, idesc, accum);
-              accum = 1;
-            }
-          }
-          umma_commit(bar);
-        }
-        __syncwarp();
+      for (int prod = 0; prod < 3; ++prod) {       // g_hi a_hi, g_lo a_hi, g_hi a_lo
+        const uint32_t gg = g_addr + (prod == 1 ? GB : 0);
+        const uint32_t aa = at_addr + (prod == 2 ? AB : 0);
+#pragma unroll
+        for (int ks = 0; ks < PXT / 8; ++ks)
+          mma_tf32<K>(d, gg + (ks >> 2) * TILE_BYTES + (ks & 3) * 32, aa + (ks >> 2) * (K * 128) + (ks & 3) * 32,
+                      (prod == 0 && ks == 0) ? 0u : 1u);
       }
-      mbar_wait(bar, phase);
-      phase ^= 1;
-      tc_fence_after();
-      if (half == 0) {                      // warps 0-1 of the warpgroup own TMEM lanes 0..63 = rows (pos, f) < 64
+      wg::commit();
+      wg::wait<0>();
+      wg::fence_regs(d);
 #pragma unroll
-        for (int c0 = 0; c0 < K; c0 += 16) {
-          float t[16];
-          tmem_ld16(tmem_row + (uint32_t)c0, t);
-          tmem_ld_wait();
-#pragma unroll
-          for (int e = 0; e < 16; ++e) acc[c0 + e] += t[e];
-        }
-      }
-      tc_fence_before();
+      for (int k = 0; k < K / 2; ++k) acc[k] += d[k];
+      wg_barrier(wg);                      // every warp's MMAs are done before the operands are rebuilt
     }
     __syncthreads();
   }
   // ---- fold: dump dW' and the bias sums to shared memory (the operand tiles are free now), then fixed-order sums ----
-  tc_fence_before();
   __syncthreads();
   float* s_d = reinterpret_cast<float*>(base);                  // [2 wg][64 rows][K]
   float* s_db = s_d + 2 * 64 * K;                               // [2 wg][64 px][F]
-  if (half == 0) {
 #pragma unroll
-    for (int k = 0; k < K; ++k) s_d[(wg * 64 + q) * K + k] = acc[k];
-  } else {
+  for (int j = 0; j < K / 8; ++j)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int row = 16 * wq + gid + 8 * (e >> 1), k = 8 * j + 2 * tq + (e & 1);
+      s_d[(wg * 64 + row) * K + k] = acc[4 * j + e];
+    }
+  if (half == 1) {
 #pragma unroll
     for (int f = 0; f < F; ++f) s_db[(wg * 64 + q) * F + f] = accb[f];
   }
@@ -571,22 +411,16 @@ conv_stem_tc_bwd_kernel(const float* __restrict__ images, const uint32_t* __rest
     for (int i = 0; i < 2 * 64; ++i) sum += s_db[i * F + f];
     mine[K9 * F + f] = sum;
   }
-  __syncthreads();
-  if (warp == 0) {
-    __syncwarp();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)TMEM_COLS)
-                 : "memory");
-  }
 }
 
 template <int CIN, int F>
 static size_t bwd_smem_bytes(int h, int w) {
   constexpr int K = 16 * CIN;
-  return 1024 + (size_t)2 * (2 * 2 * TILE_BYTES + 2 * 2 * K * 128) + (size_t)2 * (h + 2) * (w + 2) * CIN * 4 + 2 * 8 + 16;
+  return 1024 + (size_t)2 * (2 * 2 * TILE_BYTES + 2 * 2 * K * 128) + (size_t)2 * (h + 2) * (w + 2) * CIN * 4;
 }
 
 bool bwd_supported(int h, int w, int cin, int f) {
-  if (f != 16) return false;               // (pos, f) rows must fit TMEM lanes 0..63 of the drainer warps
+  if (f != 16) return false;               // (pos, f) rows are the 64 rows of one wgmma
   const size_t smem = cin == 3 ? bwd_smem_bytes<3, 16>(h, w) : bwd_smem_bytes<1, 16>(h, w);
   return smem <= 227 * 1024;
 }
@@ -614,7 +448,7 @@ template <int CIN, int F>
 static size_t smem_bytes(int h, int w) {
   constexpr int K = 16 * CIN, KB = (K + 31) / 32, N = 4 * F;
   return 1024 + (size_t)2 * KB * N * 128 + (size_t)2 * 2 * KB * TILE_BYTES +
-         (size_t)fwd_image_buffers(F) * (h + 2) * (w + 2) * CIN * 4 + F * 4 + 8 * 8 + 16;
+         (size_t)fwd_image_buffers(F) * (h + 2) * (w + 2) * CIN * 4 + F * 4;
 }
 
 template <int CIN, int F>
@@ -624,7 +458,7 @@ static int launch(const float* images, const float* kernel, const float* bias, c
   auto kern = conv_stem_tc_fwd_kernel<CIN, F>;
   const int64_t cap = sm_count();
   const int grid = (int)(batch < cap ? batch : cap);
-  kern<<<grid, FWD_THREADS, smem, st>>>(images, kernel, bias, pv, pl::overflow_flag(), argmax, batch, h, w);
+  kern<<<grid, THREADS, smem, st>>>(images, kernel, bias, pv, pl::overflow_flag(), argmax, batch, h, w);
   ADN_CHECK_LAUNCH("conv_stem_tc_fwd");
   return ADN_OK;
 }
@@ -639,7 +473,7 @@ int init() {
   return ADN_OK;
 }
 
-// true when the tcgen05 path covers the shape (else the caller takes the SIMT kernel)
+// true when the tensor-core path covers the shape (else the caller takes the SIMT kernel)
 bool supported(int h, int w, int cin, int f) {
   if (f != 16 && f != 32) return false;
   const size_t smem = cin == 3 ? (f == 16 ? smem_bytes<3, 16>(h, w) : smem_bytes<3, 32>(h, w))

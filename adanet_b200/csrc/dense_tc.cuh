@@ -1,4 +1,4 @@
-// tcgen05 (5th-gen tensor core) 3xTF32 dense path: TMA-fed, TMEM accumulators.
+// Tensor-core split-plane dense path (planes.cu): TMA-fed wgmma / mma.sync, register accumulators.
 // See dense_tc.cu for the design.  Entry points mirror dense_simt.cuh.
 #pragma once
 #include "common.cuh"

@@ -3,7 +3,7 @@
 // (pass 1), re-read from L2 for the mixture-weight gradient (pass 2), with
 // coalesced float4 loads over the flat [rows*dim] tile of each member.
 //
-// Reference arithmetic being replaced (file:line under /root/reference):
+// Reference arithmetic being replaced (file:line in tensorflow/adanet v0.9.0):
 //   weighted logits / sum    adanet/ensemble/weighted.py:433-453,545-561
 //   head loss                adanet/core/ensemble_builder.py:416-420,571-583
 //   complexity regulariser   adanet/ensemble/weighted.py:351-358,563-604

@@ -1,11 +1,11 @@
-// Split-plane tensor formats of the tcgen05 dense pipeline (planes.cu) and the helpers every kernel that
+// Split-plane tensor formats of the tensor-core dense pipeline (planes.cu) and the helpers every kernel that
 // WRITES planes shares (GEMM epilogues, head loss, optimizer, conv stem).
 //
 // A matrix T[rows, cols] (fp32) is held as two planes of 11-significant-bit values plus sign bits:
 //
 //   ADN_PLANES_F16  (default)  hi = fp16(T)        lo' = fp16((T - hi) * 2^11)       T ~= hi + 2^-11 lo'
 //       2 B / value, k-block = 64 columns (one 128 B swizzle row), plane[cols/64][rows][64]
-//       GEMMs issue tcgen05.mma.kind::f16 (twice the kind::tf32 rate):
+//       GEMMs issue fp16 wgmma (twice the tf32 rate):
 //           H = sum a_hi b_hi,   S = sum (a_hi b_lo' + a_lo' b_hi),   C = H + 2^-11 S
 //       fp16 carries 5 exponent bits: full 22-bit precision for 2^-14 <= |T| < 65504, absolute error 2^-36
 //       below that; gradient tensors (O(1/batch)) are therefore carried multiplied by a power of two
@@ -15,7 +15,7 @@
 //       its output planes and surfaces as a non-finite loss.  Either way the host re-runs the iteration on TF32
 //       planes (core/search.py restart_on_tf32_if_overflowed).
 //   ADN_PLANES_TF32            hi = rna_tf32(T)    lo  = rna_tf32(T - hi)            T ~= hi + lo
-//       4 B / value, k-block = 32 columns, plane[cols/32][rows][32]; kind::tf32 MMAs; fp32 exponent range.
+//       4 B / value, k-block = 32 columns, plane[cols/32][rows][32]; tf32 MMAs; fp32 exponent range.
 //
 // Both: hi plane, lo plane, then sign bits  bits[ceil(cols/32)][rows]  (uint32, bit j = T[row, 32 q + j] > 0).
 // The K padding (columns up to the k-block multiple) is zero.

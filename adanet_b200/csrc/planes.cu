@@ -1,38 +1,33 @@
-// Plane-native tcgen05 dense pipeline: fp32-accurate GEMMs whose operands AND results live in HBM as
+// Plane-native dense pipeline on Hopper tensor cores: fp32-accurate GEMMs whose operands AND results live in HBM as
 // pre-split hi/lo planes (plane_fmt.cuh), so no conversion pass sits between the layers of a subnetwork.
 //
 // Two plane formats share one kernel template:
 //   FMT_F16  (default)  hi = fp16(T), lo' = fp16((T - hi) 2^11); 2 B / value, k-block = 64 columns;
-//                       tcgen05.mma.kind::f16, C = sum a_hi b_hi + 2^-11 sum (a_hi b_lo' + a_lo' b_hi)
+//                       wgmma m64n64k16 f16, C = sum a_hi b_hi + 2^-11 sum (a_hi b_lo' + a_lo' b_hi)
 //   FMT_TF32 (fallback) hi = rna_tf32(T), lo = rna_tf32(T - hi); 4 B / value, k-block = 32 columns;
-//                       tcgen05.mma.kind::tf32, C = sum a_hi b_hi + sum (a_hi b_lo + a_lo b_hi)
+//                       mma.sync m16n8k8 tf32, C = sum a_hi b_hi + sum (a_hi b_lo + a_lo b_hi)
 // Both carry 22 significant bits per value and drop only the lo*lo term (2^-22 relative).
 //
 // Planes of T[rows, cols] are k-block-major  plane[cols/BK][rows][BK]  (one 128 B row per (k-block, row)),
 // zero padded in cols, followed by sign bits  bits[cols/32][rows]  (the ReLU mask of the backward pass costs
 // 1/32..1/16 of a plane instead of a 4 B/element read).  One layout serves every GEMM of training because
-// tcgen05 takes either operand K-major or MN-major straight from shared memory:
-//     K  = cols of T : box {BK, 128 rows, 1 kb}        -> K-major  [128 rows][BK]           SWIZZLE_128B
-//     K  = rows of T : box {BK, BK rows, 128/BK kb}    -> MN-major [128/BK][BK k][BK mn]    SWIZZLE_128B (f16)
-//                                                                                           SWIZZLE_128B_ATOM_32B (tf32)
-//   all boxes are 16 KiB.
+// TMA can cut an operand tile out of the planes in either majorness:
+//     K  = cols of T : box {BK, R rows, 1 kb}      -> K-major  [R rows][BK]          SWIZZLE_128B
+//     K  = rows of T : box {BK, BK rows, R/BK kb}  -> MN-major [R/BK][BK k][BK mn]   SWIZZLE_128B
+//   R = 128 for the A operand (tile rows), 64 for the B operand (tile columns).
 //     fwd  Y = X W       A = Xp  K-major (K=in)    B = Wp  MN-major (N=out, K=in)
 //     dX   = dZ W^T      A = dZp K-major (K=out)   B = Wp  K-major  (N=in,  K=out)
 //     dW   = X^T dZ      A = Xp  MN-major (M=in)   B = dZp MN-major (N=out), K = batch
 //   -> no transposed copies, and the epilogue of one GEMM writes the planes the
 //   next one reads (bias+ReLU for fwd, ReLU mask + column sums for dX).
+// wgmma takes fp16 operands in either majorness (the transpose bits of the instruction); its tf32 form takes K-major
+// operands only, so the TF32 planes are multiplied with mma.sync from fragments read out of the same swizzled tiles.
 //
-// The tensor core truncates its fp32 accumulator on every add, so hi*hi partial sums stay in TMEM for
-// 128 K only and are then added in registers with RN (profiles/r1a_accuracy_probe_*.txt,
-// profiles/r2a_proto_f16.txt); cross terms use their own accumulator.
+// The tensor core's fp32 accumulation does not round to nearest, so hi*hi partial sums are kept in the MMA
+// accumulator for 128 K only and then added into a separate register accumulator with RN; cross terms likewise.
 //
-// Kernel: persistent, one CTA per SM, 576 threads, warp-specialised, grouped (up to 8 GEMMs per launch)
-//   warp 0    TMA producer (3-stage ring, 64 KiB per stage: A_hi A_lo B_hi B_lo)
-//   warp 1    MMA issuer (elected lane; per K step one N=256 MMA a_hi x [b_hi|b_lo] + one N=128 MMA a_lo x b_hi)
-//   warps 2-17 epilogue (TMEM lane quadrant = warp % 4, column group = (warp-2)/4, 32 accumulators each):
-//             tcgen05.ld -> registers (bias/ReLU/dropout + sign bits | sign-bit mask + column sums) -> hi/lo split
-//             -> planes out: the warp's 2 KB smem slab + one TMA store per plane ([32 rows][32 columns] box);
-//                dense fp32 out (logits, dW partials): per-warp swizzled smem transpose -> full-sector stores
+// Kernel (pl_gemm_kernel): persistent, grouped, 384 threads = TMA producer warpgroup + 2 consumer warpgroups of 64
+// rows of a 128 x 64 tile; epilogues run row-per-lane after a shared-memory transpose, plane tiles leave by TMA.
 //
 // Reference arithmetic replaced: tf.layers.dense and its gradients,
 //   adanet/examples/simple_dnn.py:72-86,103-110.
@@ -51,42 +46,36 @@
 
 #include "dense_simt.cuh"
 #include "planes.cuh"
+#include "wgmma.cuh"
 
 namespace adn {
 namespace pl {
 
-static constexpr int BM = 128, BN = 128;
+static constexpr int BM = 128, BN = 64;
 static constexpr int STAGES = 3;
-static constexpr int TILE_BYTES = 128 * 128;          // 16 KiB: 128 rows x one 128 B k-block row
-static constexpr int STAGE_BYTES = 4 * TILE_BYTES;    // A_hi A_lo B_hi B_lo
-// 16 epilogue warps x 32 columns (TMEM lane quadrant = warp % 4, column group = (warp-2)/4): the short-K layer
-// waves are bound by epilogue latency per warp, so thread-level parallelism is what helps; each warp stages
-// 32x16 floats (2 KB) at a time to stay inside the 32 KB left beside the 3-stage ring.
-static constexpr int EPI_WARPS = 16;
-static constexpr int NUM_THREADS = 64 + 32 * EPI_WARPS;
+static constexpr int A_TILE = BM * 128;               // 16 KiB: 128 rows x one 128 B k-block row
+static constexpr int B_TILE = BN * 128;               // 8 KiB
+static constexpr int STAGE_BYTES = 2 * A_TILE + 2 * B_TILE;   // A_hi A_lo B_hi B_lo
+static constexpr int CONSUMERS = 2;                   // consumer warpgroups, 64 tile rows each
+static constexpr int EPI_WARPS = 4 * CONSUMERS;
+static constexpr int NUM_THREADS = 128 * (1 + CONSUMERS);
+static constexpr int ACC_LD = BN + 4;                 // padded row of a warpgroup's [64][BN] accumulator staging tile
+static constexpr int ACC_BYTES = CONSUMERS * 64 * ACC_LD * 4;
+// each epilogue warp stages 32x16 floats (2 KB) at a time: the plane slab of the TMA stores / the dense transpose
 static constexpr int EPI_STAGE_FLOATS = 32 * 16;
 static constexpr int EPI_BYTES = EPI_WARPS * EPI_STAGE_FLOATS * 4;
 static constexpr int BAR_BYTES = 256;
-static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + EPI_BYTES + BAR_BYTES;
-static constexpr int TMEM_COLS = 512;                 // two chunk buffers of [H: 128 | S: 128] columns
+static constexpr int SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + ACC_BYTES + EPI_BYTES + BAR_BYTES;   // (+ alignment)
 static constexpr int MAX_SPLITS = 64;
 
 template <int FMT> struct Fmt;
 template <> struct Fmt<FMT_TF32> {
   static constexpr int BK = 32;          // columns per k-block (128 B)
-  static constexpr int CHUNK = 4;        // k-blocks per TMEM accumulation chunk (K = 128)
-  static constexpr uint32_t MN_STEP = 1024u >> 4;   // descriptor address advance per MMA, MN-major operand (8 k rows)
-  static constexpr uint32_t MN_LBO = 4096u >> 4;    // next 32-wide mn block
-  static constexpr uint32_t MN_HI = (uint32_t)(512 >> 4) | (1u << 14) | (1u << 29);   // SBO 512, SWIZZLE_128B_BASE32B
-  static constexpr uint32_t IDESC_AB = (2u << 7) | (2u << 10);                        // a = b = TF32
+  static constexpr int CHUNK = 4;        // k-blocks per accumulation chunk (K = 128)
 };
 template <> struct Fmt<FMT_F16> {
   static constexpr int BK = 64;
   static constexpr int CHUNK = 2;        // K = 128
-  static constexpr uint32_t MN_STEP = 2048u >> 4;   // 16 k rows
-  static constexpr uint32_t MN_LBO = 8192u >> 4;    // next 64-wide mn block
-  static constexpr uint32_t MN_HI = (uint32_t)(1024 >> 4) | (1u << 14) | (2u << 29);  // SBO 1024, SWIZZLE_128B
-  static constexpr uint32_t IDESC_AB = 0u;                                            // a = b = F16
 };
 
 enum { EPI_BIAS_ACT = 0, EPI_MASK = 1, EPI_PARTIAL = 2 };
@@ -178,80 +167,6 @@ __device__ __forceinline__ void sts_v4(uint32_t addr, uint32_t a, uint32_t b, ui
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// Shared-memory matrix descriptor (cute::UMMA::SmemDescriptor):
-//   [0,14) start address >> 4 | [16,30) LBO >> 4 | [32,46) SBO >> 4 | [46,48) version = 1 | [61,64) layout type
-//   K-major  tile [128 rows][128 B of k], SWIZZLE_128B (type 2): SBO = 1024 (8 rows x 128 B), LBO unused (=1);
-//            next MMA (K = 8 tf32 / 16 f16): +32 B
-//   MN-major tile [128/BK mn-blocks][BK k][BK mn] (each k row 128 B):
-//     f16 : SWIZZLE_128B (type 2), atom = 64 mn x 8 k rows: LBO = 8192 (next 64-wide mn block), SBO = 1024
-//           (next 8 k rows); next MMA (16 k rows): +2048 B
-//     tf32: 32-bit MN-major operands must use the 32 B-granular 128 B swizzle SWIZZLE_128B_BASE32B (type 1, TMA
-//           CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B; atom = 32 mn x 4 k rows): LBO = 4096, SBO = 512; next MMA
-//           (8 k rows): +1024 B
-static constexpr uint32_t K_MAJOR_HI = (uint32_t)(1024 >> 4) | (1u << 14) | (2u << 29);
-template <int FMT>
-__device__ __forceinline__ uint32_t desc_hi_word(int mn_major) { return mn_major ? Fmt<FMT>::MN_HI : K_MAJOR_HI; }
-template <int FMT>
-__device__ __forceinline__ uint32_t desc_lo_word(uint32_t smem_addr, int mn_major) {
-  return ((smem_addr & 0x3FFFFu) >> 4) | ((mn_major ? Fmt<FMT>::MN_LBO : 1u) << 16);
-}
-// Instruction descriptor (cute::UMMA::InstrDescriptor): c=F32 [4,6)=1, a format [7,10), b format [10,13)
-// (0 = F16, 2 = TF32), a_major [15], b_major [16] (0 = K, 1 = MN), n_dim=N>>3 [17,23), m_dim=M>>4 [24,29).
-template <int FMT>
-__device__ __forceinline__ uint32_t make_idesc(int m, int n, int a_mn, int b_mn) {
-  return (1u << 4) | Fmt<FMT>::IDESC_AB | ((uint32_t)a_mn << 15) | ((uint32_t)b_mn << 16) |
-         ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
-}
-template <int FMT>
-__device__ __forceinline__ void umma(uint32_t tmem_d, uint32_t da_lo, uint32_t db_lo, uint32_t da_hi, uint32_t db_hi,
-                                     uint32_t idesc, uint32_t accum) {
-  if (FMT == FMT_F16) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-        "mov.b64 da, {%1, %3};\n\t"
-        "mov.b64 db, {%2, %4};\n\t"
-        "setp.ne.b32 p, %6, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t}"
-        ::"r"(tmem_d), "r"(da_lo), "r"(db_lo), "r"(da_hi), "r"(db_hi), "r"(idesc), "r"(accum)
-        : "memory");
-  } else {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-        "mov.b64 da, {%1, %3};\n\t"
-        "mov.b64 db, {%2, %4};\n\t"
-        "setp.ne.b32 p, %6, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], da, db, %5, p;\n\t}"
-        ::"r"(tmem_d), "r"(da_lo), "r"(db_lo), "r"(da_hi), "r"(db_hi), "r"(idesc), "r"(accum)
-        : "memory");
-  }
-}
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t.reg .pred P;\n\t"
-      "elect.sync _|P, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, P;\n\t}"
-      : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld32_nowait(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
 
 // work item -> (tile_m, tile_n, split).  n fastest so concurrently resident CTAs share A tiles.
 struct Item {
@@ -288,14 +203,14 @@ __device__ __forceinline__ uint32_t pack_h2(__half a, __half b) {
 // cbase..cbase+31).  Applies bias/ReLU (+ sign bits) or the sign-bit ReLU mask in the register layout,
 // transposes through `stage` (16 B chunks XOR-swizzled by row: conflict-free both ways) and writes with
 // lane = 4-column group of 8 rows, so every global access covers whole 32 B sectors.
-__device__ __forceinline__ void st_global_v8(void* p, const uint32_t (&w)[8]) {
-  asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(p), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]),
-               "r"(w[4]), "r"(w[5]), "r"(w[6]), "r"(w[7])
-               : "memory");
+__device__ __forceinline__ void st_global_v8(void* p, const uint32_t (&w)[8]) {   // 32 B as two 16 B stores
+  uint4* q = reinterpret_cast<uint4*>(p);
+  q[0] = make_uint4(w[0], w[1], w[2], w[3]);
+  q[1] = make_uint4(w[4], w[5], w[6], w[7]);
 }
 
-// split 32 values of one row into the two planes and write them with 256-bit stores (TF32 planes, and fp16 planes
-// under ADN_PL_TMA_STORE=0; the default fp16 path is store_slice_tma_hi / _lo below)
+// split 32 values of one row into the two planes and write them with 32 B per store pair (TF32 planes, and fp16
+// planes under ADN_PL_TMA_STORE=0; the default fp16 path is store_slice_tma_hi / _lo below)
 template <int FMT>
 __device__ __forceinline__ void store_row32_planes(const GemmParams& g, const float* a, int my_row, int cbase) {
   constexpr int BK = Fmt<FMT>::BK;
@@ -335,11 +250,8 @@ __device__ __forceinline__ void store_row32_planes(const GemmParams& g, const fl
   }
 }
 
-// The same slice through shared memory and TMA (fp16 planes).  With the 256-bit stores above every lane of a store
-// instruction touches a different 128 B line, which the LSU data pipe serialises into 16 B wavefronts: 4096 of them
-// per 128x128 tile, 75 % of the pipe's cycles on the short-K layer waves (ncu l1tex__data_pipe_lsu_wavefronts,
-// profiles/r2t_epilogue_store_path.txt) and the reason the epilogue warps sat on the store scoreboard while the
-// next tile's accumulators waited.  Here a lane writes its row's 64 B of one plane into the warp's 2 KB staging
+// The same slice through shared memory and TMA (fp16 planes).  With the direct stores above every lane of a store
+// instruction touches a different 128 B line, which the load/store unit serialises into 16 B wavefronts.  Here a lane writes its row's 64 B of one plane into the warp's 2 KB staging
 // slab (16 B chunks XOR-swizzled the way CU_TENSOR_MAP_SWIZZLE_64B expects: chunk ^= (row >> 1) & 3, conflict-free)
 // and one lane hands the [32 rows][32 columns] box to the TMA unit; the lo' plane follows through the same slab once
 // the hi store has read it.  Rows past M are clipped by the tensor map.
@@ -384,9 +296,8 @@ __device__ __forceinline__ void store_slice_tma_lo(const CUtensorMap* o_lo, uint
 
 // Forward epilogue with planes out, WITHOUT a register transpose: lane = row keeps its 32 accumulators (bias already
 // added by the caller), applies ReLU / dropout, forms the sign-bit word, splits pairs of values with packed conversions
-// and hands its 32 columns of each plane to the slab + TMA store path (fp16) or writes them with 256-bit stores (TF32:
-// 128 B per plane = 4 stores).  ~10 instructions per element against ~29 of the staged path (ncu: the short-K layer
-// waves were issue-bound at 61 % issue utilisation writing 2.2 TB/s, profiles/r2e_gemm_waves_ncu_full.txt).
+// and hands its 32 columns of each plane to the slab + TMA store path (fp16) or writes them with direct 16 B stores
+// (TF32: 128 B per plane).  ~10 instructions per element against ~29 of the staged path.
 template <int FMT>
 __device__ __forceinline__ void emit_slice_fwd_planes(const GemmParams& g, float* a, int lane, int mrow0, int cbase,
                                                       const CUtensorMap* o_hi, const CUtensorMap* o_lo, uint32_t slab) {
@@ -427,7 +338,7 @@ __device__ __forceinline__ void emit_slice_fwd_planes(const GemmParams& g, float
 }
 
 // dX epilogue with planes out, without a register transpose: sign-bit ReLU mask, plane stores as in the forward
-// epilogue (slab + TMA, or 256-bit stores from the row-owning lane), and the per-32-row column sums (the bias
+// epilogue (slab + TMA, or direct stores from the row-owning lane), and the per-32-row column sums (the bias
 // gradient of the layer below) by a butterfly over the warp: at distance w a lane keeps the half of its columns selected by bit w of its lane id and receives the partner's
 // partial sums for them, so after five rounds lane l holds the sum of column l over the 32 rows (31 shuffles and
 // adds per lane, fixed order).
@@ -653,58 +564,108 @@ __device__ __forceinline__ int find_problem(const Group& grp, int cur, int item,
 }
 __device__ __forceinline__ int first_next0(const Group& grp) { return grp.n > 1 ? grp.p[1].item0 : 0x7fffffff; }
 
+__device__ __forceinline__ void wg_bar(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+
+// One k-block of a consumer warpgroup on fp16 planes: 4 K steps of 16, each hi*hi into H and hi*lo' + lo'*hi into S
+// (first: the chunk starts, the MMAs overwrite H and S).  The warpgroup's 64 A rows start 8 KiB into the A tiles in
+// both majornesses; a K step advances 32 B inside a K-major 128 B row, 16 rows of 128 B in an MN-major tile.
+template <int A_MN, int B_MN>
+__device__ __forceinline__ void f16_kblock(uint32_t st, int wgi, float (&H)[32], float (&S)[32], bool first) {
+  const uint32_t a_hi = st + (uint32_t)wgi * 8192u, a_lo = a_hi + A_TILE;
+  const uint32_t b_hi = st + 2 * A_TILE, b_lo = b_hi + B_TILE;
+  constexpr uint32_t a_step = A_MN ? 2048u : 32u, b_step = B_MN ? 2048u : 32u;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const uint32_t sd = (first && k == 0) ? 0u : 1u;
+    const uint64_t dah = wg::desc_sw128(a_hi + k * a_step), dal = wg::desc_sw128(a_lo + k * a_step);
+    const uint64_t dbh = wg::desc_sw128(b_hi + k * b_step), dbl = wg::desc_sw128(b_lo + k * b_step);
+    wg::mma_f16_n64<A_MN, B_MN>(H, dah, dbh, sd);
+    wg::mma_f16_n64<A_MN, B_MN>(S, dah, dbl, sd);
+    wg::mma_f16_n64<A_MN, B_MN>(S, dal, dbh, 1u);
+  }
+}
+
+// byte offset of (row r, byte c) in a tile of 128 B rows written by TMA with SWIZZLE_128B (16 B chunk ^= row % 8)
+__device__ __forceinline__ uint32_t sw128_off(int r, int c) {
+  return (uint32_t)(r * 128 + ((((c >> 4) ^ r) & 7) << 4) + (c & 15));
+}
+// element (mn, k) of a TF32 operand tile: K-major [rows][32 k] or MN-major [rows/32][32 k][32 mn]
+template <int MN>
+__device__ __forceinline__ uint32_t tf32_off(int mn, int k) {
+  return MN ? (uint32_t)((mn >> 5) * 4096) + sw128_off(k, 4 * (mn & 31)) : sw128_off(mn, 4 * k);
+}
+__device__ __forceinline__ void mma_tf32_16x8(float* d, const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+               "{%0, %1, %2, %3};"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+// One k-block of one consumer warp on TF32 planes: rows [arow0, +16) of the tile x all BN columns, 4 K steps of 8,
+// accumulated in the same fragment layout as the wgmma path.
+template <int A_MN, int B_MN>
+__device__ __forceinline__ void tf32_kblock(const uint8_t* st, int arow0, int lane, float (&H)[32], float (&S)[32]) {
+  const uint8_t* ah = st;
+  const uint8_t* al = st + A_TILE;
+  const uint8_t* bh = st + 2 * A_TILE;
+  const uint8_t* bl = bh + B_TILE;
+  const int gid = lane >> 2, tq = lane & 3;
+#pragma unroll
+  for (int ks = 0; ks < 4; ++ks) {
+    uint32_t fa_h[4], fa_l[4];
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const uint32_t o = tf32_off<A_MN>(arow0 + gid + 8 * (e & 1), 8 * ks + tq + 4 * (e >> 1));
+      fa_h[e] = *reinterpret_cast<const uint32_t*>(ah + o);
+      fa_l[e] = *reinterpret_cast<const uint32_t*>(al + o);
+    }
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const uint32_t o0 = tf32_off<B_MN>(8 * j + gid, 8 * ks + tq), o1 = tf32_off<B_MN>(8 * j + gid, 8 * ks + tq + 4);
+      const uint32_t bh0 = *reinterpret_cast<const uint32_t*>(bh + o0), bh1 = *reinterpret_cast<const uint32_t*>(bh + o1);
+      const uint32_t bl0 = *reinterpret_cast<const uint32_t*>(bl + o0), bl1 = *reinterpret_cast<const uint32_t*>(bl + o1);
+      mma_tf32_16x8(&H[4 * j], fa_h, bh0, bh1);
+      mma_tf32_16x8(&S[4 * j], fa_h, bl0, bl1);
+      mma_tf32_16x8(&S[4 * j], fa_l, bh0, bh1);
+    }
+  }
+}
 template <int FMT, int EPI>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 pl_gemm_kernel(const __grid_constant__ Group grp) {
   constexpr int BK = Fmt<FMT>::BK;
   constexpr int CHUNK = Fmt<FMT>::CHUNK;
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = smem_raw;
-  if ((smem_u32(smem) & 1023u) != 0u) __trap();   // SWIZZLE_128B tiles must sit on 1024 B boundaries
-  float* epi_stage = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + EPI_BYTES);
-  uint64_t* full_bar = bars;                       // [STAGES]  TMA -> MMA
-  uint64_t* empty_bar = bars + STAGES;             // [STAGES]  MMA -> TMA
-  uint64_t* acc_full = bars + 2 * STAGES;          // [2]       MMA -> epilogue (chunk ready)
-  uint64_t* acc_empty = bars + 2 * STAGES + 2;     // [2]       epilogue -> MMA (chunk drained), count EPI_WARPS
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
+  constexpr int A_MN = EPI == EPI_PARTIAL, B_MN = EPI != EPI_MASK;   // operand majorness of fwd / dX / dW
+  extern __shared__ uint8_t smem_raw[];
+  // SWIZZLE_128B tiles must sit on 1024 B boundaries
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  float* acc_stage = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);
+  float* epi_stage = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES + ACC_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + ACC_BYTES + EPI_BYTES);
+  uint64_t* full_bar = bars;                       // [STAGES]  TMA -> consumers
+  uint64_t* empty_bar = bars + STAGES;             // [STAGES]  consumers -> TMA, count EPI_WARPS
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
   const int lane = threadIdx.x & 31;
   const int n_items = grp.total_items;
 
-  if (warp == 0 && lane < grp.n) {       // every problem's descriptors: each CTA visits every problem
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(smem_u32(&full_bar[s]), 1);
+      mbar_init(smem_u32(&empty_bar[s]), EPI_WARPS);
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  if (warp == 1 && lane < grp.n) {       // every problem's descriptors: each CTA visits every problem
     tma_prefetch_desc(&grp.p[lane].a_hi);
     tma_prefetch_desc(&grp.p[lane].a_lo);
     tma_prefetch_desc(&grp.p[lane].b_hi);
     tma_prefetch_desc(&grp.p[lane].b_lo);
   }
-  if (warp == 1) {
-    if (lane == 0) {
-      for (int s = 0; s < STAGES; ++s) {
-        mbar_init(smem_u32(&full_bar[s]), 1);
-        mbar_init(smem_u32(&empty_bar[s]), 1);
-      }
-      for (int b = 0; b < 2; ++b) {
-        mbar_init(smem_u32(&acc_full[b]), 1);
-        mbar_init(smem_u32(&acc_empty[b]), EPI_WARPS);
-      }
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "r"((uint32_t)TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ================= TMA producer =================
-    if (lane == 0) {
+    if (warp == 0 && lane == 0) {
       uint32_t s = 0, ph = 0;
       int cur = 0, next0 = first_next0(grp);
       const uint32_t smem0 = smem_u32(smem);
@@ -719,513 +680,116 @@ pl_gemm_kernel(const __grid_constant__ Group grp) {
           mbar_expect_tx(fb, STAGE_BYTES);
           const uint32_t base = smem0 + s * STAGE_BYTES;
           const int kc = it.kb0 + kb;
-          // K-major box {BK, 128 rows, 1 kb} at (0, row0, kc); MN-major box {BK, BK rows, 128/BK kb} at (0, kc*BK, mn0/BK)
-          const int a1 = g.a_mn ? kc * BK : it.m0, a2 = g.a_mn ? (it.m0 / BK) : kc;
-          const int b1 = g.b_mn ? kc * BK : it.n0, b2 = g.b_mn ? (it.n0 / BK) : kc;
-          tma_load_3d(&pr.a_hi, fb, base + 0 * TILE_BYTES, 0, a1, a2);
-          tma_load_3d(&pr.a_lo, fb, base + 1 * TILE_BYTES, 0, a1, a2);
-          tma_load_3d(&pr.b_hi, fb, base + 2 * TILE_BYTES, 0, b1, b2);
-          tma_load_3d(&pr.b_lo, fb, base + 3 * TILE_BYTES, 0, b1, b2);
+          // K-major box {BK, rows, 1 kb} at (0, row0, kc); MN-major box {BK, BK rows, rows/BK kb} at (0, kc*BK, mn0/BK)
+          const int a1 = A_MN ? kc * BK : it.m0, a2 = A_MN ? (it.m0 / BK) : kc;
+          const int b1 = B_MN ? kc * BK : it.n0, b2 = B_MN ? (it.n0 / BK) : kc;
+          tma_load_3d(&pr.a_hi, fb, base, 0, a1, a2);
+          tma_load_3d(&pr.a_lo, fb, base + A_TILE, 0, a1, a2);
+          tma_load_3d(&pr.b_hi, fb, base + 2 * A_TILE, 0, b1, b2);
+          tma_load_3d(&pr.b_lo, fb, base + 2 * A_TILE + B_TILE, 0, b1, b2);
           if (++s == STAGES) { s = 0; ph ^= 1; }
         }
       }
     }
-  } else if (warp == 1) {
-    // ================= MMA issuer =================
-    // The warp runs the loop converged (all lanes wait on the barriers); only the issue is under
-    // elect.sync, so every operand is warp-uniform.  The issue loop keeps ring counters incremental and
-    // builds descriptors from 32-bit halves.
-    {
-      const uint32_t smem0 = smem_u32(smem);
-      uint32_t s = 0, ph = 0, gchunk = 0;
-      int cur = 0, next0 = first_next0(grp);
-      for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-        cur = find_problem(grp, cur, item, next0);
-        const GemmParams& g = grp.p[cur].g;
-        const Item it = decode_item(g, item - grp.p[cur].item0);
-        // B_hi and B_lo tiles are adjacent in the stage, so ONE N=256 MMA computes a_hi x [b_hi | b_lo] (hi*hi into
-        // columns [0,128), hi*lo into [128,256) of the chunk buffer) and a second N=128 MMA adds a_lo x b_hi to the
-        // cross-term half: 20 KiB of operand reads per K step instead of 24 (the 128x128 single-CTA tile is
-        // bound by shared-memory traffic, not by MMA issue), same 192 clk of tensor work.
-        const uint32_t idesc256 = make_idesc<FMT>(BM, 2 * BN, g.a_mn, g.b_mn);
-        const uint32_t idesc128 = make_idesc<FMT>(BM, BN, g.a_mn, g.b_mn);
-        const uint32_t dah = desc_hi_word<FMT>(g.a_mn), dbh = desc_hi_word<FMT>(g.b_mn);
-        const uint32_t a_lo0 = desc_lo_word<FMT>(smem0, g.a_mn);
-        const uint32_t b_lo0 = desc_lo_word<FMT>(smem0 + 2 * TILE_BYTES, g.b_mn);
-        const uint32_t a_step = g.a_mn ? Fmt<FMT>::MN_STEP : (32u >> 4);   // address-field advance per MMA
-        const uint32_t b_step = g.b_mn ? Fmt<FMT>::MN_STEP : (32u >> 4);
-        for (int kb = 0; kb < it.nkb; kb += CHUNK, ++gchunk) {
-          const uint32_t b = gchunk & 1;
-          mbar_wait(smem_u32(&acc_empty[b]), ((gchunk >> 1) & 1) ^ 1);      // chunk buffer drained
-          tc_fence_after();
-          const uint32_t acc = tmem_base + b * 256;     // [H: 128 cols | S: 128 cols]
-          const int nk = min(CHUNK, it.nkb - kb);
-          uint32_t accum = 0;                      // first MMA of the chunk overwrites both halves
-          for (int kk = 0; kk < nk; ++kk) {
-            mbar_wait(smem_u32(&full_bar[s]), ph);
-            tc_fence_after();
-            const uint32_t so = s * (STAGE_BYTES >> 4);
-            if (elect_one()) {
+    return;
+  }
+
+  // ================= consumer warpgroups 1..2 =================
+  const int wgi = warp / 4 - 1;                    // which 64 rows of the tile
+  const int wq = warp & 3;                         // warp inside the warpgroup
+  const int gid = lane >> 2, tq = lane & 3;        // accumulator fragment coordinates
+  float* my_acc = acc_stage + wgi * 64 * ACC_LD;
+  float* stage = epi_stage + (warp - 4) * EPI_STAGE_FLOATS;
+  const uint32_t smem0 = smem_u32(smem);
+  uint32_t s = 0, ph = 0;
+  int cur = 0, next0 = first_next0(grp);
+  float H[32], S[32];
 #pragma unroll
-              for (int k = 0; k < 4; ++k) {          // 4 MMAs per 128 B k-block (K = 8 tf32 / 16 f16 each)
-                const uint32_t a_hi = a_lo0 + so + k * a_step, a_lo = a_hi + (TILE_BYTES >> 4);
-                const uint32_t b_hi = b_lo0 + so + k * b_step;
-                umma<FMT>(acc, a_hi, b_hi, dah, dbh, idesc256, (k == 0) ? accum : 1u);       // hi*hi | hi*lo
-                umma<FMT>(acc + 128, a_lo, b_hi, dah, dbh, idesc128, 1u);                    // + lo*hi
-              }
-              umma_commit(smem_u32(&empty_bar[s]));  // frees this smem stage when the MMAs retire
-              if (kk == nk - 1) umma_commit(smem_u32(&acc_full[b]));   // chunk complete
-            }
-            __syncwarp();
-            accum = 1u;
-            if (++s == STAGES) { s = 0; ph ^= 1; }
-          }
+  for (int j = 0; j < 32; ++j) H[j] = S[j] = 0.f;
+  for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+    cur = find_problem(grp, cur, item, next0);
+    const GemmParams& g = grp.p[cur].g;
+    const Item it = decode_item(g, item - grp.p[cur].item0);
+    float acc[32];
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {       // the bias starts the accumulation
+        const int col = it.n0 + 8 * j + 2 * tq + (e & 1);
+        acc[4 * j + e] = (EPI == EPI_BIAS_ACT && g.bias && col < g.N) ? __ldg(g.bias + col) : 0.f;
+      }
+    for (int kb = 0; kb < it.nkb; ++kb) {
+      const bool first = (kb % CHUNK) == 0;
+      const bool last = (kb % CHUNK) == CHUNK - 1 || kb == it.nkb - 1;
+      mbar_wait(smem_u32(&full_bar[s]), ph);
+      if (FMT == FMT_F16) {
+        wg::fence_regs(H);
+        wg::fence_regs(S);
+        wg::fence();
+        f16_kblock<A_MN, B_MN>(smem0 + s * STAGE_BYTES, wgi, H, S, first);
+        wg::commit();
+        wg::wait<0>();
+        wg::fence_regs(H);
+        wg::fence_regs(S);
+      } else {
+        if (first) {
+#pragma unroll
+          for (int j = 0; j < 32; ++j) H[j] = S[j] = 0.f;
         }
+        tf32_kblock<A_MN, B_MN>(smem + s * STAGE_BYTES, 64 * wgi + 16 * wq, lane, H, S);
       }
-    }
-  } else {
-    // ================= epilogue warps 2..17 =================
-    const int quad = warp & 3;                       // TMEM lane quadrant a warp may read = warp % 4
-    const int cgrp = (warp - 2) >> 2;                // which 32 of the tile's 128 columns
-    const uint32_t lane_base = (uint32_t)(quad * 32) << 16;
-    const uint32_t col_base = (uint32_t)(cgrp * 32);
-    float* stage = epi_stage + (warp - 2) * EPI_STAGE_FLOATS;
-    uint32_t gchunk = 0;
-    int cur = 0, next0 = first_next0(grp);
-    for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-      cur = find_problem(grp, cur, item, next0);
-      const GemmParams& g = grp.p[cur].g;
-      const Item it = decode_item(g, item - grp.p[cur].item0);
-      const int mrow0 = it.m0 + quad * 32;
-      const int ncol0 = it.n0 + (int)col_base;        // first output column of this warp
-      const int my_row = mrow0 + lane;
-      // ReLU mask: one sign-bit word per (row, 32-column block), fetched before the accumulators are awaited
-      uint32_t mw = 0xffffffffu;
-      if (EPI == EPI_MASK && g.mask_bits) {
-        const int kbo = ncol0 >> 5;
-        mw = (my_row < g.M && kbo < g.out_nb32) ? __ldg(g.mask_bits + (size_t)kbo * g.M + my_row) : 0u;
-      }
-      float acc[32];
-      if (EPI == EPI_BIAS_ACT && g.bias) {
-        // the bias starts the accumulation (fetched while the first chunk is still in flight): warp-uniform loads
-        if (ncol0 + 32 <= g.N && (reinterpret_cast<uintptr_t>(g.bias) & 15) == 0) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(smem_u32(&empty_bar[s]));     // this warp is done with the stage
+      if (++s == STAGES) { s = 0; ph ^= 1; }
+      if (last) {
 #pragma unroll
-          for (int jj = 0; jj < 8; ++jj) {
-            const float4 bv = __ldg(reinterpret_cast<const float4*>(g.bias + ncol0) + jj);
-            acc[4 * jj + 0] = bv.x; acc[4 * jj + 1] = bv.y;
-            acc[4 * jj + 2] = bv.z; acc[4 * jj + 3] = bv.w;
-          }
+        for (int j = 0; j < 32; ++j) acc[j] += H[j];   // fp32 RN adds
+        if (FMT == FMT_F16) {
+#pragma unroll
+          for (int j = 0; j < 32; ++j) acc[j] = fmaf(S[j], 1.0f / 2048.0f, acc[j]);   // lo' carries 2^11
         } else {
 #pragma unroll
-          for (int j = 0; j < 32; ++j) acc[j] = (ncol0 + j < g.N) ? __ldg(g.bias + ncol0 + j) : 0.f;
-        }
-      } else {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) acc[j] = 0.f;
-      }
-      const int nchunks = (it.nkb + CHUNK - 1) / CHUNK;
-      for (int c = 0; c < nchunks; ++c, ++gchunk) {
-        const uint32_t b = gchunk & 1;
-        mbar_wait(smem_u32(&acc_full[b]), (gchunk >> 1) & 1);
-        tc_fence_after();
-        {
-          uint32_t r0[32], r1[32];
-          tmem_ld32_nowait(tmem_base + lane_base + b * 256 + col_base, r0);          // hi*hi partial sums of this chunk
-          tmem_ld32_nowait(tmem_base + lane_base + b * 256 + 128 + col_base, r1);    // cross terms of this chunk
-          tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 32; ++j) acc[j] += __uint_as_float(r0[j]);   // fp32 RN adds
-          if (FMT == FMT_F16) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) acc[j] = fmaf(__uint_as_float(r1[j]), 1.0f / 2048.0f, acc[j]);   // lo' carries 2^11
-          } else {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) acc[j] += __uint_as_float(r1[j]);
-          }
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(smem_u32(&acc_empty[b]));
-      }
-      // ---- tile output: this warp's 32 rows x 32 columns ----
-      float* dense = reinterpret_cast<float*>(g.out);
-      if (EPI == EPI_PARTIAL) dense += (size_t)it.split * g.M * g.N;
-      const bool out_planes = g.out_planes != 0;
-      const bool dense_vec = !out_planes && ((g.ldc & 3) == 0) && ((reinterpret_cast<uintptr_t>(dense) & 15) == 0);
-      const int rows_ok = min(32, g.M - mrow0);          // warp-uniform; <= 0: nothing to write
-      if (FMT == FMT_F16) {     // the previous slice's TMA store must have read the staging slab
-        if (lane == 0) bulk_wait_read0();
-        __syncwarp();
-      }
-      emit_slice<FMT, EPI>(g, out_planes, acc, mw, stage, lane, mrow0, ncol0, rows_ok, dense, dense_vec, true,
-                           &grp.p[cur].o_hi, &grp.p[cur].o_lo);
-    }
-    if (FMT == FMT_F16 && lane == 0) bulk_wait0();    // stores complete before the CTA (and its shared memory) goes away
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)TMEM_COLS)
-                 : "memory");
-  }
-}
-
-// ---------------------------------------------------------------------------------
-// CTA-pair GEMM kernel (tcgen05 cta_group::2): one 256 x 256 tile per pair of SMs, grouped like pl_gemm_kernel.
-//
-// With fp16 planes the tensor pipe retires a 128 B k-block of the 128x128 single-CTA tile in 768 clk while that
-// tile needs 64 KiB of operands for it: 85 B/clk per SM out of L2 (21 TB/s chip-wide at the cuBLAS fp16 rate) and
-// a 3-stage ring that covers only ~0.9 us of TMA latency -- profiles/r2e_gemm_single_ncu_full.txt shows the
-// tensor pipe 55-59 % active with nothing else saturated.  The pair tile moves (128 A rows + 128 B rows) per SM for
-// twice the tensor work: half the L2 and shared-memory traffic per flop, twice the latency cover per stage.
-//   CTA rank r of the pair owns A rows / D rows [m0 + 128 r, +128) and supplies B rows
-//   [n0 + r n_inst/2, + n_inst/2); the leader (rank 0) issues tcgen05.mma.cta_group::2 (M = 256,
-//   N = n_inst <= 256, trimmed to the live columns) for both SMs.
-//   TMEM per SM (512 columns): H [0,256) = hi*hi partial sums of ONE 128-K chunk, S [256,512) = cross
-//   terms of the whole tile.  H is single-buffered: the next chunk starts with its cross-term MMAs
-//   while the epilogue warps of both CTAs drain H into registers.
-//   Barriers: TMA of both CTAs -> leader's full[s] (tx bytes of both); commit multicast -> both CTAs'
-//   empty[s] / acc_full; epilogue warps of both CTAs -> leader's acc_empty / s_empty (remote arrive).
-// ---------------------------------------------------------------------------------
-static constexpr int BM2 = 256, BN2 = 256;
-static constexpr int EPI_WARPS2 = 16;              // 4 TMEM lane quadrants x 4 column groups of 64: the single-buffered H must be
-static constexpr int NUM_THREADS2 = 64 + 32 * EPI_WARPS2;   // drained inside the cross-term window of the next chunk (1024 clk)
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ uint32_t mapa_rank(uint32_t smem_addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// Remote arrive on the leader's barrier.  Default semantics (release at CTA scope), as CUTLASS's ClusterBarrier does: what
-// these barriers hand over is TMEM state, ordered by the tcgen05 fences around them -- no generic-proxy data.  A
-// `.release.cluster` arrive instead waits for every global store the warp has in flight (the previous tile's 64 KB of
-// plane stores) and was 30 % of the kernel's stall samples (profiles/r2k_pair_kernel_ncu.txt).
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// wait on a local barrier whose arrivals come from other CTAs of the cluster: the plain (CTA-scope acquire) wait; the
-// cluster-scope acquire form compiles to an L1 invalidation (CCTL.IVALL) per successful wait
-__device__ __forceinline__ void mbar_wait_cluster(uint32_t bar, uint32_t parity) { mbar_wait(bar, parity); }
-__device__ __forceinline__ void tma_load_3d_2sm(const CUtensorMap* map, uint32_t bar_cluster, uint32_t dst, int c0, int c1,
-                                                int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar_cluster), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-template <int FMT>
-__device__ __forceinline__ void umma_2sm(uint32_t tmem_d, uint32_t da_lo, uint32_t db_lo, uint32_t da_hi, uint32_t db_hi,
-                                         uint32_t idesc, uint32_t accum) {
-  if (FMT == FMT_F16) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-        "mov.b64 da, {%1, %3};\n\t"
-        "mov.b64 db, {%2, %4};\n\t"
-        "setp.ne.b32 p, %6, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], da, db, %5, p;\n\t}"
-        ::"r"(tmem_d), "r"(da_lo), "r"(db_lo), "r"(da_hi), "r"(db_hi), "r"(idesc), "r"(accum)
-        : "memory");
-  } else {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-        "mov.b64 da, {%1, %3};\n\t"
-        "mov.b64 db, {%2, %4};\n\t"
-        "setp.ne.b32 p, %6, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::tf32 [%0], da, db, %5, p;\n\t}"
-        ::"r"(tmem_d), "r"(da_lo), "r"(db_lo), "r"(da_hi), "r"(db_hi), "r"(idesc), "r"(accum)
-        : "memory");
-  }
-}
-__device__ __forceinline__ void umma_commit_2sm(uint32_t bar) {   // arrives on the barrier at this offset in BOTH CTAs
-  asm volatile(
-      "{\n\t.reg .b16 m;\n\tmov.b16 m, 3;\n\t"
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], m;\n\t}"
-      ::"r"(bar)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld16_nowait(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-}
-
-struct Item2 {
-  int m0, n0, kb0, nkb, split, n_inst;
-};
-template <int FMT>
-__device__ __forceinline__ Item2 decode_item2(const GemmParams& g, int item) {
-  Item2 it;
-  it.split = (g.splits == 1) ? 0 : fast_div(item, g.inv_tiles);      // 256 x 256 tiles
-  const int t = item - it.split * g.tiles;
-  const int tm = (g.tiles_n == 1) ? t : fast_div(t, g.inv_tiles_n);
-  it.m0 = tm * BM2;
-  it.n0 = (t - tm * g.tiles_n) * BN2;
-  it.kb0 = it.split * g.kb_per_split;
-  it.nkb = min(g.total_kb, it.kb0 + g.kb_per_split) - it.kb0;
-  // live columns in steps of 2 k-block widths: each CTA's half must start on a k-block boundary of an MN-major B
-  constexpr int GR = 2 * Fmt<FMT>::BK;
-  it.n_inst = min(BN2, ((g.N - it.n0 + GR - 1) / GR) * GR);
-  return it;
-}
-
-template <int FMT, int EPI>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NUM_THREADS2, 1)
-pl_gemm2_kernel(const __grid_constant__ Group grp) {
-  constexpr int BK = Fmt<FMT>::BK;
-  constexpr int CHUNK = Fmt<FMT>::CHUNK;
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = smem_raw;
-  if ((smem_u32(smem) & 1023u) != 0u) __trap();
-  float* epi_stage = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + EPI_BYTES);
-  uint64_t* full_bar = bars;                       // [STAGES]  leader's: TMA of both CTAs -> MMA
-  uint64_t* empty_bar = bars + STAGES;             // [STAGES]  each CTA's: MMA commit (multicast) -> TMA
-  uint64_t* acc_full = bars + 2 * STAGES;          // [1]       each CTA's: MMA commit (multicast) -> epilogue
-  uint64_t* acc_empty = bars + 2 * STAGES + 1;     // [1]       leader's: epilogue warps of both CTAs -> MMA (H drained)
-  uint64_t* s_empty = bars + 2 * STAGES + 2;       // [1]       leader's: epilogue warps of both CTAs -> MMA (S drained)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 3);
-
-  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const int pair = blockIdx.x >> 1, npairs = gridDim.x >> 1;
-  const int n_items = grp.total_items;
-
-  if (warp == 0 && lane < grp.n) {
-    tma_prefetch_desc(&grp.p[lane].a_hi);
-    tma_prefetch_desc(&grp.p[lane].a_lo);
-    tma_prefetch_desc(&grp.p[lane].b_hi);
-    tma_prefetch_desc(&grp.p[lane].b_lo);
-  }
-  if (warp == 1) {
-    if (lane == 0) {
-      for (int s = 0; s < STAGES; ++s) {
-        mbar_init(smem_u32(&full_bar[s]), 1);
-        mbar_init(smem_u32(&empty_bar[s]), 1);
-      }
-      mbar_init(smem_u32(acc_full), 1);
-      mbar_init(smem_u32(acc_empty), 2 * EPI_WARPS2);
-      mbar_init(smem_u32(s_empty), 2 * EPI_WARPS2);
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "r"((uint32_t)TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();          // both CTAs' barriers are initialised before any remote arrive / multicast commit
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 0) {
-    // ================= TMA producer (both CTAs: own A rows, own half of B) =================
-    if (lane == 0) {
-      uint32_t s = 0, ph = 0;
-      int cur = 0, next0 = first_next0(grp);
-      const uint32_t smem0 = smem_u32(smem);
-      for (int item = pair; item < n_items; item += npairs) {
-        cur = find_problem(grp, cur, item, next0);
-        const Problem& pr = grp.p[cur];
-        const GemmParams& g = pr.g;
-        const Item2 it = decode_item2<FMT>(g, item - pr.item0);
-        const int a_row = it.m0 + (int)rank * 128;
-        const int b_row = it.n0 + (int)rank * (it.n_inst >> 1);
-        for (int kb = 0; kb < it.nkb; ++kb) {
-          mbar_wait(smem_u32(&empty_bar[s]), ph ^ 1);
-          if (rank == 0) mbar_expect_tx(smem_u32(&full_bar[s]), 2 * STAGE_BYTES);   // bytes of both CTAs
-          const uint32_t fb = mapa_rank(smem_u32(&full_bar[s]), 0);                 // leader's barrier
-          const uint32_t base = smem0 + s * STAGE_BYTES;
-          const int kc = it.kb0 + kb;
-          const int a1 = g.a_mn ? kc * BK : a_row, a2 = g.a_mn ? (a_row / BK) : kc;
-          const int b1 = g.b_mn ? kc * BK : b_row, b2 = g.b_mn ? (b_row / BK) : kc;
-          tma_load_3d_2sm(&pr.a_hi, fb, base + 0 * TILE_BYTES, 0, a1, a2);
-          tma_load_3d_2sm(&pr.a_lo, fb, base + 1 * TILE_BYTES, 0, a1, a2);
-          tma_load_3d_2sm(&pr.b_hi, fb, base + 2 * TILE_BYTES, 0, b1, b2);
-          tma_load_3d_2sm(&pr.b_lo, fb, base + 3 * TILE_BYTES, 0, b1, b2);
-          if (++s == STAGES) { s = 0; ph ^= 1; }
+          for (int j = 0; j < 32; ++j) acc[j] += S[j];
         }
       }
     }
-  } else if (warp == 1) {
-    // ================= MMA issuer (leader CTA only) =================
-    if (rank == 0) {
-      const uint32_t smem0 = smem_u32(smem);
-      const uint32_t acc_h = tmem_base, acc_s = tmem_base + 256;
-      uint32_t s = 0, ph = 0, gchunk = 0, tile_i = 0;
-      int cur = 0, next0 = first_next0(grp);
-      for (int item = pair; item < n_items; item += npairs, ++tile_i) {
-        cur = find_problem(grp, cur, item, next0);
-        const GemmParams& g = grp.p[cur].g;
-        const Item2 it = decode_item2<FMT>(g, item - grp.p[cur].item0);
-        const uint32_t dah = desc_hi_word<FMT>(g.a_mn), dbh = desc_hi_word<FMT>(g.b_mn);
-        const uint32_t a_lo0 = desc_lo_word<FMT>(smem0, g.a_mn);
-        const uint32_t b_lo0 = desc_lo_word<FMT>(smem0 + 2 * TILE_BYTES, g.b_mn);
-        const uint32_t a_step = g.a_mn ? Fmt<FMT>::MN_STEP : (32u >> 4);
-        const uint32_t b_step = g.b_mn ? Fmt<FMT>::MN_STEP : (32u >> 4);
-        const uint32_t idesc = make_idesc<FMT>(BM2, it.n_inst, g.a_mn, g.b_mn);
-        mbar_wait_cluster(smem_u32(s_empty), (tile_i & 1) ^ 1);     // cross-term accumulator drained by both CTAs
-        tc_fence_after();
-        uint32_t s_accum = 0;
-        for (int kb = 0; kb < it.nkb; kb += CHUNK, ++gchunk) {
-          const int nk = min(CHUNK, it.nkb - kb);
-          for (int kk = 0; kk < nk; ++kk) {
-            mbar_wait(smem_u32(&full_bar[s]), ph);
-            tc_fence_after();
-            const uint32_t so = s * (STAGE_BYTES >> 4);
-            if (kk == 0) {
-              // new chunk: cross terms first, so the tensor pipe stays busy while H is being drained
-              if (elect_one()) {
+    // ---- fragment layout -> row per lane: the warpgroup's [64][BN] tile through shared memory ----
+    wg_bar(1 + wgi);                               // the previous tile's rows have been read
 #pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                  const uint32_t a_hi = a_lo0 + so + k * a_step, a_lo = a_hi + (TILE_BYTES >> 4);
-                  const uint32_t b_hi = b_lo0 + so + k * b_step, b_lo = b_hi + (TILE_BYTES >> 4);
-                  umma_2sm<FMT>(acc_s, a_lo, b_hi, dah, dbh, idesc, (k == 0) ? s_accum : 1u);
-                  umma_2sm<FMT>(acc_s, a_hi, b_lo, dah, dbh, idesc, 1u);
-                }
-              }
-              __syncwarp();
-              mbar_wait_cluster(smem_u32(acc_empty), (gchunk & 1) ^ 1);   // H drained by both CTAs
-              tc_fence_after();
-              if (elect_one()) {
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                  const uint32_t a_hi = a_lo0 + so + k * a_step;
-                  const uint32_t b_hi = b_lo0 + so + k * b_step;
-                  umma_2sm<FMT>(acc_h, a_hi, b_hi, dah, dbh, idesc, (k == 0) ? 0u : 1u);
-                }
-                umma_commit_2sm(smem_u32(&empty_bar[s]));
-                if (nk == 1) umma_commit_2sm(smem_u32(acc_full));
-              }
-            } else {
-              if (elect_one()) {
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                  const uint32_t a_hi = a_lo0 + so + k * a_step, a_lo = a_hi + (TILE_BYTES >> 4);
-                  const uint32_t b_hi = b_lo0 + so + k * b_step, b_lo = b_hi + (TILE_BYTES >> 4);
-                  umma_2sm<FMT>(acc_s, a_lo, b_hi, dah, dbh, idesc, 1u);
-                  umma_2sm<FMT>(acc_s, a_hi, b_lo, dah, dbh, idesc, 1u);
-                  umma_2sm<FMT>(acc_h, a_hi, b_hi, dah, dbh, idesc, 1u);
-                }
-                umma_commit_2sm(smem_u32(&empty_bar[s]));
-                if (kk == nk - 1) umma_commit_2sm(smem_u32(acc_full));
-              }
-            }
-            __syncwarp();
-            s_accum = 1u;
-            if (++s == STAGES) { s = 0; ph ^= 1; }
-          }
-        }
-      }
+    for (int j = 0; j < 8; ++j) {
+      const int row = 16 * wq + gid, col = 8 * j + 2 * tq;
+      *reinterpret_cast<float2*>(my_acc + row * ACC_LD + col) = make_float2(acc[4 * j], acc[4 * j + 1]);
+      *reinterpret_cast<float2*>(my_acc + (row + 8) * ACC_LD + col) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
     }
-  } else {
-    // ================= epilogue warps 2..17 (both CTAs; 32 rows x 64 columns each) =================
-    const int quad = warp & 3;
-    const int cgrp = (warp - 2) >> 2;                // which 64 of the tile's 256 columns
-    const uint32_t lane_base = (uint32_t)(quad * 32) << 16;
-    const uint32_t col_base = (uint32_t)(cgrp * 64);
-    float* stage = epi_stage + (warp - 2) * EPI_STAGE_FLOATS;
-    const uint32_t acc_empty_leader = mapa_rank(smem_u32(acc_empty), 0);
-    const uint32_t s_empty_leader = mapa_rank(smem_u32(s_empty), 0);
-    uint32_t gchunk = 0;
-    int cur = 0, next0 = first_next0(grp);
-    for (int item = pair; item < n_items; item += npairs) {
-      cur = find_problem(grp, cur, item, next0);
-      const GemmParams& g = grp.p[cur].g;
-      const Item2 it = decode_item2<FMT>(g, item - grp.p[cur].item0);
-      const int mrow0 = it.m0 + (int)rank * 128 + quad * 32;
-      const int ncol0 = it.n0 + (int)col_base;
-      const int my_row = mrow0 + lane;
-      const bool cols_live = (int)col_base < it.n_inst;   // warp-uniform: does this warp own any computed column?
-      uint32_t mw[2] = {0xffffffffu, 0xffffffffu};
-      if (EPI == EPI_MASK && g.mask_bits) {
+    wg_bar(1 + wgi);
+    const int rs = 32 * (wq & 1), cs = 32 * (wq >> 1);
 #pragma unroll
-        for (int q = 0; q < 2; ++q) {
-          const int kbo = (ncol0 >> 5) + q;
-          mw[q] = (my_row < g.M && kbo < g.out_nb32) ? __ldg(g.mask_bits + (size_t)kbo * g.M + my_row) : 0u;
-        }
-      }
-      float acc[64];
-#pragma unroll
-      for (int j = 0; j < 64; ++j) acc[j] = 0.f;
-      const int nchunks = (it.nkb + CHUNK - 1) / CHUNK;
-      for (int c = 0; c < nchunks; ++c, ++gchunk) {
-        mbar_wait(smem_u32(acc_full), gchunk & 1);
-        tc_fence_after();
-        if (cols_live) {
-#pragma unroll
-          for (int t = 0; t < 2; ++t) {
-            uint32_t r0[32];
-            tmem_ld32_nowait(tmem_base + lane_base + col_base + t * 32, r0);
-            tmem_ld_wait();
-#pragma unroll
-            for (int j = 0; j < 32; ++j) acc[t * 32 + j] += __uint_as_float(r0[j]);   // fp32 RN adds
-          }
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive_cluster(acc_empty_leader);      // H may be overwritten: the next chunk's hi*hi MMAs
-        if (c == nchunks - 1) {
-          if (cols_live) {
-#pragma unroll
-            for (int t = 0; t < 2; ++t) {
-              uint32_t r0[32];
-              tmem_ld32_nowait(tmem_base + lane_base + 256 + col_base + t * 32, r0);
-              tmem_ld_wait();
-#pragma unroll
-              for (int j = 0; j < 32; ++j) {
-                if (FMT == FMT_F16) acc[t * 32 + j] = fmaf(__uint_as_float(r0[j]), 1.0f / 2048.0f, acc[t * 32 + j]);
-                else acc[t * 32 + j] += __uint_as_float(r0[j]);
-              }
-            }
-          }
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive_cluster(s_empty_leader);
-        }
-      }
-      if (cols_live) {
-        float* dense = reinterpret_cast<float*>(g.out);
-        if (EPI == EPI_PARTIAL) dense += (size_t)it.split * g.M * g.N;
-        const bool out_planes = g.out_planes != 0;
-        const bool dense_vec = !out_planes && ((g.ldc & 3) == 0) && ((reinterpret_cast<uintptr_t>(dense) & 15) == 0);
-        const int rows_ok = min(32, g.M - mrow0);
-#pragma unroll
-        for (int q = 0; q < 2; ++q)
-          if ((int)col_base + q * 32 < it.n_inst) {
-            if (EPI == EPI_BIAS_ACT && g.bias) {       // the direct epilogues expect the bias inside the accumulators
-              const int cb = ncol0 + q * 32;
-#pragma unroll
-              for (int j = 0; j < 32; ++j) acc[q * 32 + j] += (cb + j < g.N) ? __ldg(g.bias + cb + j) : 0.f;
-            }
-            emit_slice<FMT, EPI>(g, out_planes, &acc[q * 32], mw[q], stage, lane, mrow0, ncol0 + q * 32, rows_ok, dense,
-                                 dense_vec, true);
-          }
-      }
+    for (int q = 0; q < 8; ++q) {
+      const float4 v = *reinterpret_cast<const float4*>(my_acc + (rs + lane) * ACC_LD + cs + 4 * q);
+      acc[4 * q] = v.x; acc[4 * q + 1] = v.y; acc[4 * q + 2] = v.z; acc[4 * q + 3] = v.w;
     }
+    // ---- tile output: this warp's 32 rows x 32 columns ----
+    const int mrow0 = it.m0 + 64 * wgi + rs;
+    const int ncol0 = it.n0 + cs;
+    const int my_row = mrow0 + lane;
+    uint32_t mw = 0xffffffffu;                     // ReLU mask: one sign-bit word per (row, 32-column block)
+    if (EPI == EPI_MASK && g.mask_bits) {
+      const int kbo = ncol0 >> 5;
+      mw = (my_row < g.M && kbo < g.out_nb32) ? __ldg(g.mask_bits + (size_t)kbo * g.M + my_row) : 0u;
+    }
+    float* dense = reinterpret_cast<float*>(g.out);
+    if (EPI == EPI_PARTIAL) dense += (size_t)it.split * g.M * g.N;
+    const bool out_planes = g.out_planes != 0;
+    const bool dense_vec = !out_planes && ((g.ldc & 3) == 0) && ((reinterpret_cast<uintptr_t>(dense) & 15) == 0);
+    const int rows_ok = min(32, g.M - mrow0);          // warp-uniform; <= 0: nothing to write
+    if (FMT == FMT_F16) {     // the previous slice's TMA store must have read the staging slab
+      if (lane == 0) bulk_wait_read0();
+      __syncwarp();
+    }
+    emit_slice<FMT, EPI>(g, out_planes, acc, mw, stage, lane, mrow0, ncol0, rows_ok, dense, dense_vec, true,
+                         &grp.p[cur].o_hi, &grp.p[cur].o_lo);
   }
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();          // neither CTA frees TMEM / exits while the peer may still use its smem or barriers
-  if (warp == 1) {
-    __syncwarp();
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)TMEM_COLS)
-                 : "memory");
-  }
+  if (FMT == FMT_F16 && lane == 0) bulk_wait0();    // stores complete before the CTA (and its shared memory) goes away
 }
 
 // ---------------------------------------------------------------------------------
@@ -1364,11 +928,6 @@ int init() {
     ADN_PL_ATTR(FMT_TF32, EPI_BIAS_ACT); ADN_PL_ATTR(FMT_TF32, EPI_MASK); ADN_PL_ATTR(FMT_TF32, EPI_PARTIAL);
     ADN_PL_ATTR(FMT_F16, EPI_BIAS_ACT); ADN_PL_ATTR(FMT_F16, EPI_MASK); ADN_PL_ATTR(FMT_F16, EPI_PARTIAL);
 #undef ADN_PL_ATTR
-#define ADN_PL_ATTR2(F, E) \
-  ok = ok && (cudaFuncSetAttribute(pl_gemm2_kernel<F, E>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) == cudaSuccess)
-    ADN_PL_ATTR2(FMT_TF32, EPI_BIAS_ACT); ADN_PL_ATTR2(FMT_TF32, EPI_MASK); ADN_PL_ATTR2(FMT_TF32, EPI_PARTIAL);
-    ADN_PL_ATTR2(FMT_F16, EPI_BIAS_ACT); ADN_PL_ATTR2(FMT_F16, EPI_MASK); ADN_PL_ATTR2(FMT_F16, EPI_PARTIAL);
-#undef ADN_PL_ATTR2
     if (!ok) {
       (void)cudaGetLastError();
       rc = fail(ADN_ERR_CUDA, "pl::init: cudaFuncSetAttribute(smem=%d) failed", SMEM_BYTES);
@@ -1400,17 +959,21 @@ static Operand operand(int fmt, const void* planes, int64_t rows, int64_t cols, 
 }
 
 // ---- TMA descriptor cache (include/adanet_b200.h conventions): a descriptor depends only on (plane base, rows,
-// k-blocks, majorness, format); the same few hundred recur on every eager step, eval pass and graph re-capture.
+// k-blocks, majorness, tile extent, format); the same few hundred recur on every eager step, eval pass and graph
+// re-capture.
 struct MapKey {
   const void* ptr;
   int64_t rows, nkb;
   int mn, fmt;
-  bool operator==(const MapKey& o) const { return ptr == o.ptr && rows == o.rows && nkb == o.nkb && mn == o.mn && fmt == o.fmt; }
+  int box = 0;           // tile extent of the operand (BM for A, BN for B); 0 for the store boxes
+  bool operator==(const MapKey& o) const {
+    return ptr == o.ptr && rows == o.rows && nkb == o.nkb && mn == o.mn && fmt == o.fmt && box == o.box;
+  }
 };
 struct MapKeyHash {
   size_t operator()(const MapKey& k) const {
     size_t h = reinterpret_cast<uintptr_t>(k.ptr) * 0x9E3779B97F4A7C15ull;
-    h ^= (size_t)k.rows * 0xC2B2AE3D27D4EB4Full + ((size_t)k.nkb << 20) + ((size_t)k.mn << 1) + (size_t)k.fmt;
+    h ^= (size_t)k.rows * 0xC2B2AE3D27D4EB4Full + ((size_t)k.nkb << 20) + ((size_t)k.mn << 1) + (size_t)k.fmt + ((size_t)k.box << 40);
     return h ^ (h >> 29);
   }
 };
@@ -1420,9 +983,10 @@ static std::atomic<long long> g_map_hits{0}, g_map_misses{0};
 long long map_cache_hits() { return g_map_hits.load(); }
 long long map_cache_misses() { return g_map_misses.load(); }
 
-static int make_map(int fmt, CUtensorMap* map, const void* plane, int64_t rows, int64_t nkb, int mn_major) {
+// operand tile of `box` rows (K-major) or columns (MN-major) per k-block
+static int make_map(int fmt, CUtensorMap* map, const void* plane, int64_t rows, int64_t nkb, int mn_major, int box) {
   if (!g_encode) return fail(ADN_ERR_CUDA, "pl: adn_init() was not called");
-  const MapKey key{plane, rows, nkb, mn_major, fmt};
+  const MapKey key{plane, rows, nkb, mn_major, fmt, box};
   {
     std::lock_guard<std::mutex> lk(g_map_mu);
     auto it = g_maps.find(key);
@@ -1435,10 +999,10 @@ static int make_map(int fmt, CUtensorMap* map, const void* plane, int64_t rows, 
   const int bk = fmt_bk(fmt), es = fmt_esize(fmt);
   cuuint64_t gdim[3] = {(cuuint64_t)bk, (cuuint64_t)rows, (cuuint64_t)nkb};
   cuuint64_t gstride[2] = {(cuuint64_t)bk * es, (cuuint64_t)rows * bk * es};
-  cuuint32_t box_k[3] = {(cuuint32_t)bk, 128u, 1u};
-  cuuint32_t box_mn[3] = {(cuuint32_t)bk, (cuuint32_t)bk, (cuuint32_t)(128 / bk)};
+  cuuint32_t box_k[3] = {(cuuint32_t)bk, (cuuint32_t)box, 1u};
+  cuuint32_t box_mn[3] = {(cuuint32_t)bk, (cuuint32_t)bk, (cuuint32_t)(box / bk)};
   cuuint32_t estr[3] = {1u, 1u, 1u};
-  const CUtensorMapSwizzle sw = (mn_major && fmt == FMT_TF32) ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : CU_TENSOR_MAP_SWIZZLE_128B;
+  const CUtensorMapSwizzle sw = CU_TENSOR_MAP_SWIZZLE_128B;
   CUresult r = g_encode(map, fmt == FMT_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3,
                         const_cast<void*>(plane), gdim, gstride, mn_major ? box_mn : box_k, estr,
                         CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -1480,7 +1044,7 @@ static int make_store_map(CUtensorMap* map, const void* plane, int64_t rows, int
   g_maps.emplace(key, *map);
   return ADN_OK;
 }
-static int store_mode() {      // ADN_PL_TMA_STORE=0: keep the direct 256-bit stores (A/B switch for profiles)
+static int store_mode() {      // ADN_PL_TMA_STORE=0: direct global stores instead (A/B switch)
   static const int env = getenv("ADN_PL_TMA_STORE") ? atoi(getenv("ADN_PL_TMA_STORE")) : 1;
   return env;
 }
@@ -1497,10 +1061,10 @@ static int encode_maps(int fmt, const GemmDesc& d, CUtensorMap* a_hi, CUtensorMa
        reinterpret_cast<uintptr_t>(d.b.lo)) & 127)
     return fail(ADN_ERR_INVALID, "%s: plane buffers must be 256 B aligned", what);
   int rc;
-  if ((rc = make_map(fmt, a_hi, d.a.hi, d.a.rows, d.a.nkb, d.a.mn_major))) return rc;
-  if ((rc = make_map(fmt, a_lo, d.a.lo, d.a.rows, d.a.nkb, d.a.mn_major))) return rc;
-  if ((rc = make_map(fmt, b_hi, d.b.hi, d.b.rows, d.b.nkb, d.b.mn_major))) return rc;
-  if ((rc = make_map(fmt, b_lo, d.b.lo, d.b.rows, d.b.nkb, d.b.mn_major))) return rc;
+  if ((rc = make_map(fmt, a_hi, d.a.hi, d.a.rows, d.a.nkb, d.a.mn_major, BM))) return rc;
+  if ((rc = make_map(fmt, a_lo, d.a.lo, d.a.rows, d.a.nkb, d.a.mn_major, BM))) return rc;
+  if ((rc = make_map(fmt, b_hi, d.b.hi, d.b.rows, d.b.nkb, d.b.mn_major, BN))) return rc;
+  if ((rc = make_map(fmt, b_lo, d.b.lo, d.b.rows, d.b.nkb, d.b.mn_major, BN))) return rc;
   return ADN_OK;
 }
 
@@ -1518,57 +1082,26 @@ template <int FMT, int EPI>
 static void launch_kernel(const Group& grp, int grid, cudaStream_t st) {
   pl_gemm_kernel<FMT, EPI><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(grp);
 }
-template <int FMT, int EPI>
-static void launch_kernel2(const Group& grp, int grid, cudaStream_t st) {
-  pl_gemm2_kernel<FMT, EPI><<<grid, NUM_THREADS2, SMEM_BYTES, st>>>(grp);
-}
-
-// Which GEMMs take the CTA-pair kernel.  ADN_PL_PAIR: 1 every GEMM, 2 the big ones (M, N >= 256, K >= 4 k-blocks),
-// unset / 0 none.  Measured on B200 (profiles/r2f_pair_vs_single_f16.txt): [32768,1024]x[1024,1024] fp16 planes
-// 206 us on pairs against 177 us on single CTAs (TF32 planes, round 1: equal), so the single-CTA kernel stays the
-// default and the pair kernel is kept as a tested alternative (tests force it through ADN_PL_PAIR=1).
-static int pair_mode() {
-  static const int env = getenv("ADN_PL_PAIR") ? atoi(getenv("ADN_PL_PAIR")) : 0;
-  return env;
-}
-static bool use_pair_shape(int fmt, int64_t M, int64_t N, int64_t total_kb, bool split_k = true) {
-  (void)fmt;
-  const int env = pair_mode();
-  if (env == 1) return true;
-  if (env == 2) return M >= 256 && N >= 256 && total_kb >= 4;
-  if (env == 3) return split_k && M >= 256 && N >= 256 && total_kb >= 4;     // the big dW GEMMs only
-  return false;
-}
-static bool use_pair(int fmt, const GemmDesc& d) {
-  // dropout lives in the single-CTA kernel's direct epilogue; mode 3 takes the split-K (dW) problems only
-  return d.g.drop_thresh == 0u && use_pair_shape(fmt, d.g.M, d.g.N, d.g.total_kb, d.g.out_planes == 0 && d.g.bias == nullptr &&
-                                                                                      d.g.mask_bits == nullptr && d.g.colsum_part == nullptr &&
-                                                                                      d.g.act == 0 && d.g.ldc == d.g.N && d.g.total_kb >= 64);
-}
-
-// n independent GEMMs of the same epilogue kind -> persistent launches of up to MAX_GROUP problems each; the problems
-// that take the CTA-pair kernel are launched as their own group(s)
+// n independent GEMMs of the same epilogue kind -> persistent launches of up to MAX_GROUP problems each
 template <int EPI>
 static int launch_group(int fmt, const GemmDesc* d, int n, cudaStream_t st, const char* what) {
-  for (int pass = 0; pass < 2; ++pass) {
-    const bool pair = pass == 0;
-    std::vector<int> idx;
-    for (int i = 0; i < n; ++i)
-      if (use_pair(fmt, d[i]) == pair) idx.push_back(i);
-    const int tm = pair ? BM2 : BM, tn = pair ? BN2 : BN;
-    for (size_t i0 = 0; i0 < idx.size(); i0 += MAX_GROUP) {
-      const int m = (int)std::min<size_t>(MAX_GROUP, idx.size() - i0);
+  {
+    for (int i0 = 0; i0 < n; i0 += MAX_GROUP) {
+      const int m = std::min(MAX_GROUP, n - i0);
       Group grp;
       memset(&grp, 0, sizeof(grp));
       int items = 0;
       for (int i = 0; i < m; ++i) {
-        const GemmDesc& src = d[idx[i0 + (size_t)i]];
+        const GemmDesc& src = d[i0 + i];
         Problem& pr = grp.p[i];
+        // the kernel fixes the operand majorness per epilogue kind (fwd: K / MN, dX: K / K, dW: MN / MN)
+        if (src.a.mn_major != (EPI == EPI_PARTIAL) || src.b.mn_major != (EPI != EPI_MASK))
+          return fail(ADN_ERR_INVALID, "%s: operand majorness does not match the epilogue kind", what);
         int rc = encode_maps(fmt, src, &pr.a_hi, &pr.a_lo, &pr.b_hi, &pr.b_lo, what);
         if (rc) return rc;
         pr.g = src.g;
         pr.g.out_tma = 0;
-        if (!pair && fmt == FMT_F16 && EPI != EPI_PARTIAL && src.g.out_planes && store_mode() && (src.g.out_nb32 & 1) == 0 &&
+        if (fmt == FMT_F16 && EPI != EPI_PARTIAL && src.g.out_planes && store_mode() && (src.g.out_nb32 & 1) == 0 &&
             ((reinterpret_cast<uintptr_t>(src.g.out) | reinterpret_cast<uintptr_t>(src.g.out_lo)) & 127) == 0) {
           if ((rc = make_store_map(&pr.o_hi, src.g.out, src.g.M, src.g.out_nb32 / 2))) return rc;
           if ((rc = make_store_map(&pr.o_lo, src.g.out_lo, src.g.M, src.g.out_nb32 / 2))) return rc;
@@ -1576,8 +1109,8 @@ static int launch_group(int fmt, const GemmDesc* d, int n, cudaStream_t st, cons
         }
         pr.g.a_mn = src.a.mn_major;
         pr.g.b_mn = src.b.mn_major;
-        pr.g.tiles_m = (int)ceil_div(pr.g.M, tm);
-        pr.g.tiles_n = (int)ceil_div(pr.g.N, tn);
+        pr.g.tiles_m = (int)ceil_div(pr.g.M, BM);
+        pr.g.tiles_n = (int)ceil_div(pr.g.N, BN);
         pr.g.tiles = pr.g.tiles_m * pr.g.tiles_n;
         if ((int64_t)pr.g.tiles * pr.g.splits >= (1 << 21))
           return fail(ADN_ERR_UNSUPPORTED, "%s: %d work items exceed the decode range", what, pr.g.tiles * pr.g.splits);
@@ -1591,15 +1124,9 @@ static int launch_group(int fmt, const GemmDesc* d, int n, cudaStream_t st, cons
       }
       grp.n = m;
       grp.total_items = items;
-      if (pair) {
-        const int grid = 2 * std::min(items, sm_count() / 2);
-        if (fmt == FMT_F16) launch_kernel2<FMT_F16, EPI>(grp, grid, st);
-        else launch_kernel2<FMT_TF32, EPI>(grp, grid, st);
-      } else {
-        const int grid = std::min(items, sm_count());
-        if (fmt == FMT_F16) launch_kernel<FMT_F16, EPI>(grp, grid, st);
-        else launch_kernel<FMT_TF32, EPI>(grp, grid, st);
-      }
+      const int grid = std::min(items, sm_count());
+      if (fmt == FMT_F16) launch_kernel<FMT_F16, EPI>(grp, grid, st);
+      else launch_kernel<FMT_TF32, EPI>(grp, grid, st);
       ADN_CHECK_LAUNCH(what);
     }
   }
@@ -1715,15 +1242,14 @@ int dense_bwd_group(int fmt, const BwdOp* ops, int n, int64_t batch, cudaStream_
       const double kItemOverhead = 6.0;          // k-block equivalents per work item
       const double kReduceKbPerByte = 1.0 / (2.5e6 * 0.4);     // k-block equivalents per byte of partials read
       double best_t = 1e30;
-      std::vector<double> load((size_t)workers), load2((size_t)std::max(1, workers / 2));
+      std::vector<double> load((size_t)workers);
       int64_t last_kps = -1;
       for (int s0 = 1; s0 <= MAX_SPLITS && s0 <= kb_b; ++s0) {
         const int64_t kps = ceil_div(kb_b, s0);
         if (kps == last_kps) continue;
         last_kps = kps;
         std::fill(load.begin(), load.end(), 0.0);
-        std::fill(load2.begin(), load2.end(), 0.0);
-        int64_t item = 0, item2 = 0;
+        int64_t item = 0;
         double reduce_bytes = 0.0;
         bool any = false;
         for (int i = 0; i < n; ++i) {
@@ -1731,23 +1257,15 @@ int dense_bwd_group(int fmt, const BwdOp* ops, int n, int64_t batch, cudaStream_
           any = true;
           const int64_t k_i = std::max<int64_t>(kps, ceil_div(kb_b, max_dw_splits(ops[i].in, ops[i].out)));
           const int64_t s_i = ceil_div(kb_b, k_i);
-          // problems on the CTA-pair kernel run as their own launch: 256x256 tiles on SM pairs, twice the tensor
-          // work per k-block and tile
-          const bool pair = use_pair_shape(fmt, ops[i].in, ops[i].out, kb_b);
-          const int64_t tiles = pair ? ceil_div(ops[i].in, BM2) * ceil_div(ops[i].out, BN2)
-                                     : ceil_div(ops[i].in, BM) * ceil_div(ops[i].out, BN);
+          const int64_t tiles = ceil_div(ops[i].in, BM) * ceil_div(ops[i].out, BN);
           for (int64_t sp = 0; sp < s_i; ++sp) {
             const double kb_item = (double)(std::min(kb_b, (sp + 1) * k_i) - sp * k_i);
-            if (pair) {
-              for (int64_t t = 0; t < tiles; ++t, ++item2) load2[(size_t)(item2 % (int64_t)load2.size())] += 2.0 * (kb_item + kItemOverhead);
-            } else {
-              for (int64_t t = 0; t < tiles; ++t, ++item) load[(size_t)(item % workers)] += kb_item + kItemOverhead;
-            }
+            for (int64_t t = 0; t < tiles; ++t, ++item) load[(size_t)(item % workers)] += kb_item + kItemOverhead;
           }
           if (s_i > 1) reduce_bytes += (double)(s_i + 1) * (double)ops[i].in * (double)ops[i].out * 4.0;
         }
         if (!any) break;
-        const double t = *std::max_element(load.begin(), load.end()) + *std::max_element(load2.begin(), load2.end()) +
+        const double t = *std::max_element(load.begin(), load.end()) +
                          reduce_bytes * kReduceKbPerByte + (reduce_bytes > 0 ? 10.0 : 0.0);
         if (t < best_t) { best_t = t; best_kps = kps; }
       }

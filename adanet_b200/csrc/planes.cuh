@@ -1,4 +1,4 @@
-// Plane-native tcgen05 dense pipeline (see planes.cu for the design, plane_fmt.cuh for the formats).
+// Plane-native tensor-core dense pipeline (see planes.cu for the design, plane_fmt.cuh for the formats).
 #pragma once
 #include "common.cuh"
 #include "plane_fmt.cuh"

@@ -9,7 +9,7 @@ for the 4-candidate configuration), every one the same architecture
 with he_normal kernels, constant complexity 1, a Momentum(0.9) optimizer under cosine decay of the iteration step,
 and mixture weights that are not trained (the deprecated `build_mixture_weights_train_op` returns a no-op).
 The engine runs the conv/pool/flatten stem as one fused CUDA kernel (csrc/conv_stem.cu) and the dense layers on
-the tcgen05 plane pipeline.
+the tensor-core plane pipeline.
 """
 
 from __future__ import annotations

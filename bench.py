@@ -1,13 +1,13 @@
 #!/usr/bin/env python
 """bench.py -- candidate-train examples/sec per AdaNet iteration (BASELINE.json metric).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 A "step" is one training step of EVERY candidate of the iteration on one
 minibatch (subnetwork fwd+bwd+update, candidate-ensemble head, EMA).  Workload
 (config.workload): BASELINE configs[2] -- 8-candidate DNN search 100->H->H->10,
 H in {64..1024}, 1M x 100 synthetic tabular data, B = 32768; it fits one GPU,
-so N=1 trains all 8 candidates on one B200 and N>1 places the candidates on the GPUs
+so N=1 trains all 8 candidates on one H100 and N>1 places the candidates on the GPUs
 cost-balanced, training the ones heavier than a GPU's fair share (H=1024: 46 % of the step)
 data-parallel on row slices of the minibatch over 2-4 GPUs (strong scaling: total work
 fixed; the only data-path collective is one NCCL all-reduce of such a candidate's gradient
@@ -20,8 +20,10 @@ the public adanet_b200.Estimator.train call with HOST (pinned) batches, H2D of e
 batch and a D2H read of every step's losses (an `after_run` hook) inside the timed region.
 `sustained` = the HBM-resident loop again for >= 2.5 s (power-capped steady state) with its own
 clock samples; `roofline` carries the measured cuBLAS peak of the MMA kind the kernel issues
-beside the bf16 peak of MEASURED_PEAKS.json; `cpu_baseline` = the faster of two CPU restatements
-(NumPy/OpenBLAS oracle, torch-CPU oneDNN port) on the full B=32768 minibatch.
+beside the bf16 peak of MEASURED_PEAKS.json (H100 SXM data sheet when absent); `cpu_baseline` = the faster of two
+CPU restatements (NumPy/OpenBLAS oracle, torch-CPU oneDNN port) on the full B=32768 minibatch.
+
+--dump-outputs DIR: the last timed step's losses and the iteration's trained state as float32 .npy (seeded inputs).
 """
 
 import argparse
@@ -87,7 +89,7 @@ def train_flops_per_example():
 
 
 class ClockSampler:
-  """nvidia-smi clocks/throttle reasons DURING the timed region (B200_PROFILING.md)."""
+  """nvidia-smi clocks/throttle reasons DURING the timed region."""
   Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
        "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
        "clocks_event_reasons.sw_power_cap")
@@ -135,13 +137,13 @@ class ClockSampler:
             "reasons": sorted(reasons), "samples": len(sm)}
 
 
-def load_peaks():
+def load_peaks():   # fallback: H100 SXM data sheet (700 W), HBM3 3.35 TB/s, dense BF16 989 TFLOP/s
   p = os.path.join(ROOT, "MEASURED_PEAKS.json")
   if os.path.exists(p):
     with open(p) as f:
       d = json.load(f)
-    return d.get("hbm_gbs", 6650.0), d.get("bf16_tflops", 1590.0), d.get("bf16_tflops_sustained", 1400.0), "measured"
-  return 6650.0, 1590.0, 1400.0, "fallback"
+    return d.get("hbm_gbs", 3350.0), d.get("bf16_tflops", 989.0), d.get("bf16_tflops_sustained", 989.0), "measured"
+  return 3350.0, 989.0, 989.0, "H100 SXM data sheet"
 
 
 def _cpu_arms(cores):
@@ -322,7 +324,7 @@ def measure_dominant_kernel(lib, torch, reps=20):
   xp, wp, yp = eng.new_planes(B, I, "cuda"), eng.new_planes(I, O, "cuda"), eng.new_planes(B, O, "cuda")
   _lib.check(lib.adn_planes_split(x.data_ptr(), B, I, xp.data_ptr(), sp.cuda_stream), "split")
   _lib.check(lib.adn_planes_split(w.data_ptr(), I, O, wp.data_ptr(), sp.cuda_stream), "split")
-  flush = torch.empty((256 * 1024 * 1024 // 4,), device="cuda")   # 256 MB > 126 MB L2
+  flush = torch.empty((256 * 1024 * 1024 // 4,), device="cuda")   # 256 MB > 50 MB L2
   times = []
   for i in range(reps + 3):
     flush.fill_(float(i))
@@ -334,8 +336,27 @@ def measure_dominant_kernel(lib, torch, reps=20):
     e1.synchronize()
     if i >= 3:
       times.append(e0.elapsed_time(e1) * 1e-3)
-  fmt = "f16" if _lib.plane_format() == _lib.PLANES_F16 else "tf32"
-  return float(np.mean(times)), 2.0 * B * I * O, "tcgen05_3x%s_planes" % fmt
+  f16 = _lib.plane_format() == _lib.PLANES_F16
+  return float(np.mean(times)), 2.0 * B * I * O, "wgmma_3xf16_planes" if f16 else "mma_sync_3xtf32_planes"
+
+
+def dump_outputs(dirpath, plan, limit_bytes=64 << 20, sample=1 << 21):
+  """Last step's losses + trained state as float32 .npy; arrays over `sample` elements become a fixed, seeded sample."""
+  os.makedirs(dirpath, exist_ok=True)
+  arrays = {"last_losses": plan.last_losses()}
+  for k, v in sorted(plan.state_dict().items()):
+    if np.issubdtype(np.asarray(v).dtype, np.floating):
+      arrays["state_" + k] = v
+  for name, v in arrays.items():
+    v = np.asarray(v, dtype=np.float32)
+    if v.size > sample:
+      arrays[name] = v.reshape(-1)[np.sort(np.random.default_rng(0).choice(v.size, size=sample, replace=False))]
+    else:
+      arrays[name] = v
+  if sum(v.nbytes for v in arrays.values()) > limit_bytes:    # checked before anything is written
+    raise RuntimeError("--dump-outputs: more than %d bytes" % limit_bytes)
+  for name, v in arrays.items():
+    np.save(os.path.join(dirpath, name + ".npy"), v)
 
 
 def _finish(world):
@@ -422,6 +443,8 @@ def run_ours(args):
   value = BATCH * args.steps / secs
   local_losses = plan.last_losses()
   assert np.isfinite(local_losses).all(), "non-finite loss in the timed region"
+  if args.dump_outputs and rank == 0:
+    dump_outputs(args.dump_outputs, plan)
   # ---------------- steady state: the same loop for >= 2.5 s (the chip reaches its power cap) ----------------
   sustained = None
   if not args.profile and args.sustain_seconds > 0:
@@ -560,28 +583,21 @@ def run_ours(args):
 
   # ---------------- roofline of the dominant kernel + CPU baseline (rank 0, N=1 only for cpu) ----------------
   hbm, bf16_burst, bf16_sust, which = load_peaks()
-  traffic = None   # dram bytes per launch of that kernel from the committed ncu --set full capture
-  try:
-    with open(os.path.join(ROOT, "profiles", "dominant_kernel_traffic.json")) as f:
-      traffic = int(json.load(f)["traffic_bytes"])
-  except Exception:
-    pass
   achieved = kflops / kt / 1e12
-  f16 = kpath.startswith("tcgen05_3xf16")
+  f16 = kpath.startswith("wgmma_3xf16")
   kind_peak = peaks.get("f16_tflops" if f16 else "tf32_tflops")
   plane_bytes = 2 * (2 if f16 else 4)      # hi + lo bytes per value
   roofline = {
       "bound": "tensor", "kernel": "adn_dense_fwd_p [32768,1024]x[1024,1024] bias+relu, planes in/out (%s)" % kpath,
       "achieved": achieved, "peak": bf16_burst, "unit": "TFLOP/s", "frac": achieved / bf16_burst,
-      "peak_source": "MEASURED_PEAKS.json bf16 burst (%s); numerator = algorithmic fp32 FLOPs 2*B*in*out; the tcgen05 "
+      "peak_source": "bf16 peak (%s); numerator = algorithmic fp32 FLOPs 2*B*in*out; the tensor-core "
                      "path issues 3 MMAs per product (hi*hi, hi*lo, lo*hi split for 1e-5 fp32 parity), so the design "
-                     "ceiling of `frac` is 1/3 with kind::f16 planes (1/6 with the TF32 fallback)" % which,
-      "mma_kind": "kind::f16" if f16 else "kind::tf32", "mmas_per_product": 3,
+                     "ceiling of `frac` is 1/3 with fp16 planes (1/6 with the TF32 fallback)" % which,
+      "mma_kind": "wgmma f16" if f16 else "mma.sync tf32", "mmas_per_product": 3,
       "kind_peak_measured_tflops": kind_peak, "kind_peaks_measured": peaks,
       "issued_frac_of_kind_peak": (3.0 * achieved / kind_peak) if kind_peak else None,
       "useful_frac_of_kind_peak": (achieved / kind_peak) if kind_peak else None,
-      "traffic": traffic,
-      "traffic_unit": "bytes/launch (ncu dram read+write); algorithmic: %.1f MB of split planes (%d B/value) = %.1f MB of "
+      "traffic_unit": "algorithmic: %.1f MB of split planes (%d B/value) = %.1f MB of "
                       "the fp32 tensors they represent" % ((2 * BATCH * 1024 + 1024 * 1024) * plane_bytes / 1e6, plane_bytes,
                                                            (2 * BATCH * 1024 + 1024 * 1024) * 4 / 1e6),
       "launch_seconds": kt,
@@ -614,6 +630,9 @@ def main():
   ap.add_argument("--warmup", type=int, default=5)
   ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
   ap.add_argument("--profile", action="store_true", help="step loop only (for ncu captures)")
+  ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                  help="write the last timed step's losses and trained state to DIR/<name>.npy (float32); with N > 1 "
+                       "GPUs, those of the candidates rank 0 trains")
   ap.add_argument("--sustain-seconds", type=float, default=2.5,
                   help="length of the additional steady-state measurement (0 = skip)")
   args = ap.parse_args()

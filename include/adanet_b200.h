@@ -1,11 +1,11 @@
 /*
- * adanet_b200.h -- C ABI of the B200-native AdaNet candidate-training engine.
+ * adanet_b200.h -- C ABI of the H100-native AdaNet candidate-training engine.
  *
  * The reference (tensorflow/adanet v0.9.0) has NO FFI boundary: its hot path is
  * Python that builds a TF1 graph, executed by TensorFlow's stock CPU kernels
  * (SURVEY.md section 8b).  These entry points are therefore *new*; each one
  * names the reference code whose per-step arithmetic it replaces
- * (file:line relative to /root/reference).  INTEGRATION.md shows the ctypes
+ * (file:line relative to tensorflow/adanet v0.9.0).  INTEGRATION.md shows the ctypes
  * binding a reference maintainer would add.
  *
  * Conventions
@@ -63,13 +63,13 @@ extern "C" {
 #define ADN_OPT_MOMENTUM_COSINE 4
 
 /* compute paths for the dense kernels (adn_set_dense_path / adn_query) */
-#define ADN_PATH_AUTO 0    /* tcgen05 split-plane GEMM where shapes allow, SIMT fp32 otherwise */
+#define ADN_PATH_AUTO 0    /* tensor-core split-plane GEMM where shapes allow, SIMT fp32 otherwise */
 #define ADN_PATH_SIMT 1    /* CUDA-core fp32 FMA everywhere                         */
 #define ADN_PATH_TCGEN05 2 /* force tensor path; unsupported shapes return an error  */
 
-/* split-plane formats of the tcgen05 dense pipeline (adn_set_plane_format; csrc/plane_fmt.cuh) */
-#define ADN_PLANES_TF32 0 /* hi/lo TF32, 4 B per value, kind::tf32 MMAs, fp32 exponent range           */
-#define ADN_PLANES_F16 1  /* hi/lo' fp16 (lo' carries 2^11), 2 B per value, kind::f16 MMAs (default)   */
+/* split-plane formats of the tensor-core dense pipeline (adn_set_plane_format; csrc/plane_fmt.cuh) */
+#define ADN_PLANES_TF32 0 /* hi/lo TF32, 4 B per value, tf32 MMAs, fp32 exponent range                 */
+#define ADN_PLANES_F16 1  /* hi/lo' fp16 (lo' carries 2^11), 2 B per value, fp16 MMAs (default)         */
 
 /* adn_query keys */
 #define ADN_Q_VERSION 0
@@ -111,7 +111,7 @@ int adn_plane_overflow(int* flag_host, int reset, void* stream);
  * and the forward-only replay of frozen members,
  *   adanet/core/estimator.py:1785-1882 / adanet/core/iteration.py:568-579.
  * workspace: adn_query(ADN_Q_DENSE_FWD_WORKSPACE_BYTES) bytes (hi/lo TF32 operand
- * planes of the tcgen05 path); may be NULL/0 when that query returns 0.
+ * planes of the tensor-core path); may be NULL/0 when that query returns 0.
  */
 int adn_dense_fwd(const float* x, const float* w, const float* b, float* y,
                   int64_t batch, int64_t in, int64_t out, int act,
@@ -193,7 +193,7 @@ int adn_opt_step(int kind, float* const* params_host, const float* const* grads_
  * columns; each stored k-block-major [ceil(cols/BK)][rows][BK] (zero padded in cols),
  * hi followed by lo followed by sign bits [ceil(cols/32)][rows] in one buffer of
  * adn_query(ADN_Q_PLANES_BYTES) bytes, 256 B aligned, ZERO-INITIALISED by the caller
- * once (the K padding must stay zero).  It is the operand format of the tcgen05 GEMM
+ * once (the K padding must stay zero).  It is the operand format of the tensor-core GEMM
  * (3 MMAs per product: hi*hi, hi*lo, lo*hi): the same planes are read K-major or
  * MN-major by TMA, so forward, dX and dW all consume them without a transposed copy,
  * and each GEMM's epilogue writes the planes its consumer reads.

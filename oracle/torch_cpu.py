@@ -7,7 +7,7 @@ NumPy/OpenBLAS is a weak CPU arm on a many-core host (round-1 VERDICT, weak #6);
 faster as `cpu_baseline` / `--impl reference`.  `tests/test_oracle_golden.py::test_torch_cpu_port_matches_numpy_oracle`
 pins it to `oracle/adanet_oracle.py` (which in turn is pinned to the reference's known-answer tests).
 
-Reference arithmetic restated (file:line under /root/reference):
+Reference arithmetic restated (file:line in tensorflow/adanet v0.9.0):
   dense + ReLU stack and its gradients      adanet/examples/simple_dnn.py:61-110          [TF]
   mean sparse softmax cross-entropy head    adanet/core/ensemble_builder.py:571-583       [TF]
   w * logits, complexity penalty, adanet loss, mixture-weight gradient (penalty counted twice on the

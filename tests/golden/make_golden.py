@@ -1,7 +1,7 @@
 """Generates tests/golden/*.json by importing the REFERENCE's own modules.
 
-Run in the build container only (needs /root/reference, which does not exist
-on the GPU box):   python tests/golden/make_golden.py
+Needs a checkout of tensorflow/adanet v0.9.0 (the reference):
+    python tests/golden/make_golden.py /path/to/adanet
 
 The reference is a pure-Python TF1 library; TensorFlow is not installable
 here, so only its TF-free modules can be executed:
@@ -20,7 +20,7 @@ import os
 import sys
 import types
 
-REF = "/root/reference"
+REF = sys.argv[1] if len(sys.argv) > 1 else os.environ.get("ADANET_REFERENCE", "")
 OUT = os.path.dirname(os.path.abspath(__file__))
 
 

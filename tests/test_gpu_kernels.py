@@ -1,5 +1,5 @@
 """Kernel-level parity: every C-ABI compute entry point vs the CPU oracle on the
-same seeded inputs (run on the B200 box: pytest -m gpu)."""
+same seeded inputs (run on an H100: pytest -m gpu)."""
 
 import ctypes
 

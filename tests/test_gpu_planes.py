@@ -1,5 +1,5 @@
-"""GPU parity of the plane-native tcgen05 pipeline (csrc/planes.cu) through the C ABI, in BOTH plane formats
-(fp16 hi/lo' planes with kind::f16 MMAs -- the default -- and the TF32 fallback, csrc/plane_fmt.cuh).
+"""GPU parity of the plane-native tensor-core pipeline (csrc/planes.cu) through the C ABI, in BOTH plane formats
+(fp16 hi/lo' planes with fp16 MMAs -- the default -- and the TF32 fallback, csrc/plane_fmt.cuh).
 
 Checked against fp64 NumPy restatements of the reference arithmetic
 (tf.layers.dense and its gradients, adanet/examples/simple_dnn.py:72-86,103-110)

@@ -83,7 +83,7 @@ def main():
   from tests.parity_util import orc
   B = a.batch or {2: 8192, 4: 1024, 5: 4096}[a.config]
   in_dim, C, mk, kind = build_space(a.config, a.steps + a.warmup)
-  # dataset larger than the 126 MB L2, resident in HBM
+  # dataset larger than the 50 MB L2, resident in HBM
   rows = a.rows or max(8 * B, int(2.6e8 // (4 * in_dim)) // B * B)
   g = torch.Generator(device="cuda").manual_seed(1234)
   x = (torch.rand((rows, in_dim), device="cuda", generator=g) * 2 - 1) if kind != "tabular" else \
