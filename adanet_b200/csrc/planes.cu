@@ -26,8 +26,11 @@
 // The tensor core's fp32 accumulation does not round to nearest, so hi*hi partial sums are kept in the MMA
 // accumulator for 128 K only and then added into a separate register accumulator with RN; cross terms likewise.
 //
-// Kernel (pl_gemm_kernel): persistent, grouped, 384 threads = TMA producer warpgroup + 2 consumer warpgroups of 64
-// rows of a 128 x 64 tile; epilogues run row-per-lane after a shared-memory transpose, plane tiles leave by TMA.
+// Kernel (pl_gemm_kernel): persistent, grouped, 512 threads = TMA producer warpgroup + 2 consumer warpgroups of 64
+// rows of a 128 x 64 tile + an epilogue warpgroup.  The consumers write each finished tile's accumulators into one of
+// two swizzled 32 KiB staging tiles and go on with the next tile's mainloop; the epilogue warpgroup reads the tile
+// back row-per-lane and runs bias/ReLU/dropout, masks, column sums and the stores (plane tiles leave by TMA).
+// setmaxnreg gives the producer 40 registers and the rest to the consumers and the epilogue.
 //
 // Reference arithmetic replaced: tf.layers.dense and its gradients,
 //   adanet/examples/simple_dnn.py:72-86,103-110.
@@ -57,15 +60,25 @@ static constexpr int A_TILE = BM * 128;               // 16 KiB: 128 rows x one 
 static constexpr int B_TILE = BN * 128;               // 8 KiB
 static constexpr int STAGE_BYTES = 2 * A_TILE + 2 * B_TILE;   // A_hi A_lo B_hi B_lo
 static constexpr int CONSUMERS = 2;                   // consumer warpgroups, 64 tile rows each
-static constexpr int EPI_WARPS = 4 * CONSUMERS;
-static constexpr int NUM_THREADS = 128 * (1 + CONSUMERS);
-static constexpr int ACC_LD = BN + 4;                 // padded row of a warpgroup's [64][BN] accumulator staging tile
-static constexpr int ACC_BYTES = CONSUMERS * 64 * ACC_LD * 4;
+static constexpr int CONSUMER_WARPS = 4 * CONSUMERS;
+static constexpr int EPI_WARPS = 4;                   // the epilogue warpgroup: 32 tile rows per warp
+static constexpr int NUM_THREADS = 128 * (1 + CONSUMERS) + 32 * EPI_WARPS;
+// registers per thread after setmaxnreg: 128 (40 + EPI_REGS) + 256 CONSUMER_REGS <= 65536
+static constexpr int PRODUCER_REGS = 40, EPI_REGS = 136, CONSUMER_REGS = 168;
+static_assert(128 * (PRODUCER_REGS + EPI_REGS) + 128 * CONSUMERS * CONSUMER_REGS <= 65536, "register file");
+// every warp starts with 65536 / NUM_THREADS = 128: the producer gives registers back, the others take them
+static_assert(PRODUCER_REGS < 65536 / NUM_THREADS && EPI_REGS > 65536 / NUM_THREADS &&
+              CONSUMER_REGS > 65536 / NUM_THREADS, "setmaxnreg.dec / .inc");
+// finished tiles go from the consumers to the epilogue warpgroup through ACC_BUFS [BM][BN] fp32 staging tiles
+static constexpr int ACC_BUFS = 2;
+static constexpr int ACC_TILE_FLOATS = BM * BN;
+static constexpr int ACC_BYTES = ACC_BUFS * ACC_TILE_FLOATS * 4;
 // each epilogue warp stages 32x16 floats (2 KB) at a time: the plane slab of the TMA stores / the dense transpose
 static constexpr int EPI_STAGE_FLOATS = 32 * 16;
 static constexpr int EPI_BYTES = EPI_WARPS * EPI_STAGE_FLOATS * 4;
 static constexpr int BAR_BYTES = 256;
 static constexpr int SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + ACC_BYTES + EPI_BYTES + BAR_BYTES;   // (+ alignment)
+static_assert(SMEM_BYTES <= 232448, "shared memory per block");
 static constexpr int MAX_SPLITS = 64;
 
 template <int FMT> struct Fmt;
@@ -564,7 +577,28 @@ __device__ __forceinline__ int find_problem(const Group& grp, int cur, int item,
 }
 __device__ __forceinline__ int first_next0(const Group& grp) { return grp.n > 1 ? grp.p[1].item0 : 0x7fffffff; }
 
-__device__ __forceinline__ void wg_bar(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+template <int R> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+
+// float offset of (row, col) in a [BM][BN] accumulator staging tile: 16 B chunk ^= row % 8, so that both the
+// consumers' fragment-layout float2 writes and the epilogue's row-per-lane float4 reads are bank-conflict free
+__device__ __forceinline__ int acc_off(int row, int col) {
+  return row * BN + ((((col >> 2) ^ row) & 7) | ((col >> 2) & 8)) * 4 + (col & 3);
+}
+
+// adds one 128-K chunk of the MMA accumulators into the register accumulator with fp32 RN
+template <int FMT>
+__device__ __forceinline__ void fold_chunk(float (&acc)[32], const float (&H)[32], const float (&S)[32]) {
+#pragma unroll
+  for (int j = 0; j < 32; ++j) acc[j] += H[j];
+  if (FMT == FMT_F16) {
+#pragma unroll
+    for (int j = 0; j < 32; ++j) acc[j] = fmaf(S[j], 1.0f / 2048.0f, acc[j]);   // lo' carries 2^11
+  } else {
+#pragma unroll
+    for (int j = 0; j < 32; ++j) acc[j] += S[j];
+  }
+}
 
 // One k-block of a consumer warpgroup on fp16 planes: 4 K steps of 16, each hi*hi into H and hi*lo' + lo'*hi into S
 // (first: the chunk starts, the MMAs overwrite H and S).  The warpgroup's 64 A rows start 8 KiB into the A tiles in
@@ -642,7 +676,9 @@ pl_gemm_kernel(const __grid_constant__ Group grp) {
   float* epi_stage = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES + ACC_BYTES);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + ACC_BYTES + EPI_BYTES);
   uint64_t* full_bar = bars;                       // [STAGES]  TMA -> consumers
-  uint64_t* empty_bar = bars + STAGES;             // [STAGES]  consumers -> TMA, count EPI_WARPS
+  uint64_t* empty_bar = bars + STAGES;             // [STAGES]  consumers -> TMA, count CONSUMER_WARPS
+  uint64_t* tile_full = bars + 2 * STAGES;         // [ACC_BUFS] consumers -> epilogue, count 128 CONSUMERS
+  uint64_t* tile_empty = tile_full + ACC_BUFS;     // [ACC_BUFS] epilogue -> consumers, count 32 EPI_WARPS
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
   const int lane = threadIdx.x & 31;
@@ -651,7 +687,11 @@ pl_gemm_kernel(const __grid_constant__ Group grp) {
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(smem_u32(&full_bar[s]), 1);
-      mbar_init(smem_u32(&empty_bar[s]), EPI_WARPS);
+      mbar_init(smem_u32(&empty_bar[s]), CONSUMER_WARPS);
+    }
+    for (int b = 0; b < ACC_BUFS; ++b) {
+      mbar_init(smem_u32(&tile_full[b]), 128 * CONSUMERS);
+      mbar_init(smem_u32(&tile_empty[b]), 32 * EPI_WARPS);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
@@ -665,6 +705,7 @@ pl_gemm_kernel(const __grid_constant__ Group grp) {
 
   if (warp < 4) {
     // ================= TMA producer =================
+    setmaxnreg_dec<PRODUCER_REGS>();
     if (warp == 0 && lane == 0) {
       uint32_t s = 0, ph = 0;
       int cur = 0, next0 = first_next0(grp);
@@ -694,19 +735,72 @@ pl_gemm_kernel(const __grid_constant__ Group grp) {
     return;
   }
 
+  if (warp >= 4 * (1 + CONSUMERS)) {
+    // ================= epilogue warpgroup =================
+    // Walks the same items as the consumers.  Warp ew owns tile rows [32 ew, +32): it reads each of its two 32 x 32
+    // slices back row per lane and emits it; the staging tile is released once both slices are in registers.
+    setmaxnreg_inc<EPI_REGS>();
+    const int ew = warp - 4 * (1 + CONSUMERS);
+    float* stage = epi_stage + ew * EPI_STAGE_FLOATS;
+    int cur = 0, next0 = first_next0(grp);
+    uint32_t tcount = 0;
+    for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++tcount) {
+      cur = find_problem(grp, cur, item, next0);
+      const GemmParams& g = grp.p[cur].g;
+      const Item it = decode_item(g, item - grp.p[cur].item0);
+      const uint32_t buf = tcount & 1u;
+      mbar_wait(smem_u32(&tile_full[buf]), (tcount >> 1) & 1u);
+      const float* tile = acc_stage + buf * ACC_TILE_FLOATS;
+      const int row = 32 * ew + lane;
+      const int mrow0 = it.m0 + 32 * ew;
+      const int my_row = mrow0 + lane;
+      float* dense = reinterpret_cast<float*>(g.out);
+      if (EPI == EPI_PARTIAL) dense += (size_t)it.split * g.M * g.N;
+      const bool out_planes = g.out_planes != 0;
+      const bool dense_vec = !out_planes && ((g.ldc & 3) == 0) && ((reinterpret_cast<uintptr_t>(dense) & 15) == 0);
+      const int rows_ok = min(32, g.M - mrow0);          // warp-uniform; <= 0: nothing to write
+#pragma unroll 1
+      for (int h = 0; h < 2; ++h) {
+        const int cs = 32 * h;
+        float acc[32];
+#pragma unroll
+        for (int q = 0; q < 8; ++q) {
+          const float4 v = *reinterpret_cast<const float4*>(tile + acc_off(row, cs + 4 * q));
+          acc[4 * q] = v.x; acc[4 * q + 1] = v.y; acc[4 * q + 2] = v.z; acc[4 * q + 3] = v.w;
+        }
+        if (h == 1) mbar_arrive(smem_u32(&tile_empty[buf]));
+        // ---- tile output: this warp's 32 rows x 32 columns ----
+        const int ncol0 = it.n0 + cs;
+        uint32_t mw = 0xffffffffu;                     // ReLU mask: one sign-bit word per (row, 32-column block)
+        if (EPI == EPI_MASK && g.mask_bits) {
+          const int kbo = ncol0 >> 5;
+          mw = (my_row < g.M && kbo < g.out_nb32) ? __ldg(g.mask_bits + (size_t)kbo * g.M + my_row) : 0u;
+        }
+        if (FMT == FMT_F16) {     // the previous slice's TMA store must have read the staging slab
+          if (lane == 0) bulk_wait_read0();
+          __syncwarp();
+        }
+        emit_slice<FMT, EPI>(g, out_planes, acc, mw, stage, lane, mrow0, ncol0, rows_ok, dense, dense_vec, true,
+                             &grp.p[cur].o_hi, &grp.p[cur].o_lo);
+      }
+    }
+    if (FMT == FMT_F16 && lane == 0) bulk_wait0();    // stores complete before the CTA (and its shared memory) goes away
+    return;
+  }
+
   // ================= consumer warpgroups 1..2 =================
+  setmaxnreg_inc<CONSUMER_REGS>();
   const int wgi = warp / 4 - 1;                    // which 64 rows of the tile
   const int wq = warp & 3;                         // warp inside the warpgroup
   const int gid = lane >> 2, tq = lane & 3;        // accumulator fragment coordinates
-  float* my_acc = acc_stage + wgi * 64 * ACC_LD;
-  float* stage = epi_stage + (warp - 4) * EPI_STAGE_FLOATS;
   const uint32_t smem0 = smem_u32(smem);
   uint32_t s = 0, ph = 0;
   int cur = 0, next0 = first_next0(grp);
-  float H[32], S[32];
+  uint32_t tcount = 0;
+  float H[32], S[32];                              // MMA accumulators of one 128-K chunk
 #pragma unroll
   for (int j = 0; j < 32; ++j) H[j] = S[j] = 0.f;
-  for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+  for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++tcount) {
     cur = find_problem(grp, cur, item, next0);
     const GemmParams& g = grp.p[cur].g;
     const Item it = decode_item(g, item - grp.p[cur].item0);
@@ -741,55 +835,20 @@ pl_gemm_kernel(const __grid_constant__ Group grp) {
       __syncwarp();
       if (lane == 0) mbar_arrive(smem_u32(&empty_bar[s]));     // this warp is done with the stage
       if (++s == STAGES) { s = 0; ph ^= 1; }
-      if (last) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) acc[j] += H[j];   // fp32 RN adds
-        if (FMT == FMT_F16) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) acc[j] = fmaf(S[j], 1.0f / 2048.0f, acc[j]);   // lo' carries 2^11
-        } else {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) acc[j] += S[j];
-        }
-      }
+      if (last) fold_chunk<FMT>(acc, H, S);
     }
-    // ---- fragment layout -> row per lane: the warpgroup's [64][BN] tile through shared memory ----
-    wg_bar(1 + wgi);                               // the previous tile's rows have been read
+    // ---- hand the tile to the epilogue warpgroup: fragment layout into staging tile tcount % 2 ----
+    const uint32_t buf = tcount & 1u;
+    mbar_wait(smem_u32(&tile_empty[buf]), ((tcount >> 1) & 1u) ^ 1u);
+    float* tile = acc_stage + buf * ACC_TILE_FLOATS;
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
-      const int row = 16 * wq + gid, col = 8 * j + 2 * tq;
-      *reinterpret_cast<float2*>(my_acc + row * ACC_LD + col) = make_float2(acc[4 * j], acc[4 * j + 1]);
-      *reinterpret_cast<float2*>(my_acc + (row + 8) * ACC_LD + col) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+      const int row = 64 * wgi + 16 * wq + gid, col = 8 * j + 2 * tq;
+      *reinterpret_cast<float2*>(tile + acc_off(row, col)) = make_float2(acc[4 * j], acc[4 * j + 1]);
+      *reinterpret_cast<float2*>(tile + acc_off(row + 8, col)) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
     }
-    wg_bar(1 + wgi);
-    const int rs = 32 * (wq & 1), cs = 32 * (wq >> 1);
-#pragma unroll
-    for (int q = 0; q < 8; ++q) {
-      const float4 v = *reinterpret_cast<const float4*>(my_acc + (rs + lane) * ACC_LD + cs + 4 * q);
-      acc[4 * q] = v.x; acc[4 * q + 1] = v.y; acc[4 * q + 2] = v.z; acc[4 * q + 3] = v.w;
-    }
-    // ---- tile output: this warp's 32 rows x 32 columns ----
-    const int mrow0 = it.m0 + 64 * wgi + rs;
-    const int ncol0 = it.n0 + cs;
-    const int my_row = mrow0 + lane;
-    uint32_t mw = 0xffffffffu;                     // ReLU mask: one sign-bit word per (row, 32-column block)
-    if (EPI == EPI_MASK && g.mask_bits) {
-      const int kbo = ncol0 >> 5;
-      mw = (my_row < g.M && kbo < g.out_nb32) ? __ldg(g.mask_bits + (size_t)kbo * g.M + my_row) : 0u;
-    }
-    float* dense = reinterpret_cast<float*>(g.out);
-    if (EPI == EPI_PARTIAL) dense += (size_t)it.split * g.M * g.N;
-    const bool out_planes = g.out_planes != 0;
-    const bool dense_vec = !out_planes && ((g.ldc & 3) == 0) && ((reinterpret_cast<uintptr_t>(dense) & 15) == 0);
-    const int rows_ok = min(32, g.M - mrow0);          // warp-uniform; <= 0: nothing to write
-    if (FMT == FMT_F16) {     // the previous slice's TMA store must have read the staging slab
-      if (lane == 0) bulk_wait_read0();
-      __syncwarp();
-    }
-    emit_slice<FMT, EPI>(g, out_planes, acc, mw, stage, lane, mrow0, ncol0, rows_ok, dense, dense_vec, true,
-                         &grp.p[cur].o_hi, &grp.p[cur].o_lo);
+    mbar_arrive(smem_u32(&tile_full[buf]));
   }
-  if (FMT == FMT_F16 && lane == 0) bulk_wait0();    // stores complete before the CTA (and its shared memory) goes away
 }
 
 // ---------------------------------------------------------------------------------
