@@ -30,6 +30,9 @@
 // rows of a 128 x 64 tile + an epilogue warpgroup.  The consumers write each finished tile's accumulators into one of
 // two swizzled 32 KiB staging tiles and go on with the next tile's mainloop; the epilogue warpgroup reads the tile
 // back row-per-lane and runs bias/ReLU/dropout, masks, column sums and the stores (plane tiles leave by TMA).
+// The epilogue is the pace-setter of the thin-K waves, so its per-tile chain is kept short: the accumulators stay in
+// registers, the global words a tile needs (ReLU mask, dropout step) are loaded one work item ahead, and each warp
+// has a hi and a lo' store slab, so a slice never waits for a TMA store it has just issued.
 // setmaxnreg gives the producer 40 registers and the rest to the consumers and the epilogue.
 //
 // Reference arithmetic replaced: tf.layers.dense and its gradients,
@@ -73,9 +76,10 @@ static_assert(PRODUCER_REGS < 65536 / NUM_THREADS && EPI_REGS > 65536 / NUM_THRE
 static constexpr int ACC_BUFS = 2;
 static constexpr int ACC_TILE_FLOATS = BM * BN;
 static constexpr int ACC_BYTES = ACC_BUFS * ACC_TILE_FLOATS * 4;
-// each epilogue warp stages 32x16 floats (2 KB) at a time: the plane slab of the TMA stores / the dense transpose
+// each epilogue warp has two 2 KB slabs (32x16 floats): the hi and the lo' plane slab of the TMA stores, so that a
+// slice's two stores go out back to back; the first slab also serves the dense transpose
 static constexpr int EPI_STAGE_FLOATS = 32 * 16;
-static constexpr int EPI_BYTES = EPI_WARPS * EPI_STAGE_FLOATS * 4;
+static constexpr int EPI_BYTES = EPI_WARPS * 2 * EPI_STAGE_FLOATS * 4;
 static constexpr int BAR_BYTES = 256;
 static constexpr int SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + ACC_BYTES + EPI_BYTES + BAR_BYTES;   // (+ alignment)
 static_assert(SMEM_BYTES <= 232448, "shared memory per block");
@@ -172,6 +176,8 @@ __device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, uint32_t sr
 }
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// all but the most recently committed store group have finished reading shared memory
+__device__ __forceinline__ void bulk_wait_read1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void sts_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
@@ -266,13 +272,13 @@ __device__ __forceinline__ void store_row32_planes(const GemmParams& g, const fl
 // The same slice through shared memory and TMA (fp16 planes).  With the direct stores above every lane of a store
 // instruction touches a different 128 B line, which the load/store unit serialises into 16 B wavefronts.  Here a lane writes its row's 64 B of one plane into the warp's 2 KB staging
 // slab (16 B chunks XOR-swizzled the way CU_TENSOR_MAP_SWIZZLE_64B expects: chunk ^= (row >> 1) & 3, conflict-free)
-// and one lane hands the [32 rows][32 columns] box to the TMA unit; the lo' plane follows through the same slab once
-// the hi store has read it.  Rows past M are clipped by the tensor map.
-// Two phases so that the caller can put independent work (sign bits, column sums) between the hi store's issue and the
-// wait for it to have read the slab: phase 1 returns the packed lo' words.
-__device__ __forceinline__ void store_slice_tma_hi(const CUtensorMap* o_hi, uint32_t slab, const float* a, int lane, int mrow0,
-                                                   int cbase, uint32_t (&lw)[16]) {
-  uint32_t w[16];
+// and one lane hands the [32 rows][32 columns] box to the TMA unit.  Rows past M are clipped by the tensor map.
+// The hi and lo' planes have a slab each, and every slice commits its hi store and then its lo' store, so before a
+// slab is written `wait_group.read 1` only waits for the store issued from it one slice earlier, not for the one
+// just issued.
+__device__ __forceinline__ void store_slice_tma(const CUtensorMap* o_hi, const CUtensorMap* o_lo, uint32_t slab_hi,
+                                                uint32_t slab_lo, const float* a, int lane, int mrow0, int cbase) {
+  uint32_t w[16], lw[16];
 #pragma unroll
   for (int q = 0; q < 16; ++q) {
     const __half2 h2 = __floats2half2_rn(a[2 * q], a[2 * q + 1]);
@@ -281,28 +287,25 @@ __device__ __forceinline__ void store_slice_tma_hi(const CUtensorMap* o_hi, uint
     w[q] = *reinterpret_cast<const uint32_t*>(&h2);
     lw[q] = *reinterpret_cast<const uint32_t*>(&l2);
   }
-  const uint32_t row = slab + (uint32_t)lane * 64u, sw = ((uint32_t)lane >> 1) & 3u;
-  // (the caller made sure the slab is free: bulk_wait_read0 + __syncwarp before the slice)
+  const uint32_t roff = (uint32_t)lane * 64u, sw = ((uint32_t)lane >> 1) & 3u;
+  if (lane == 0) bulk_wait_read1();        // the hi store of the previous slice has read slab_hi
+  __syncwarp();
 #pragma unroll
-  for (uint32_t j = 0; j < 4; ++j) sts_v4(row + ((j ^ sw) << 4), w[4 * j], w[4 * j + 1], w[4 * j + 2], w[4 * j + 3]);
+  for (uint32_t j = 0; j < 4; ++j) sts_v4(slab_hi + roff + ((j ^ sw) << 4), w[4 * j], w[4 * j + 1], w[4 * j + 2], w[4 * j + 3]);
   fence_async_smem();
   __syncwarp();
   if (lane == 0) {
-    tma_store_3d(o_hi, slab, cbase & 63, mrow0, cbase >> 6);
+    tma_store_3d(o_hi, slab_hi, cbase & 63, mrow0, cbase >> 6);
     bulk_commit();
+    bulk_wait_read1();                     // the lo' store of the previous slice has read slab_lo
   }
-}
-__device__ __forceinline__ void store_slice_tma_lo(const CUtensorMap* o_lo, uint32_t slab, const uint32_t (&lw)[16], int lane,
-                                                   int mrow0, int cbase) {
-  const uint32_t row = slab + (uint32_t)lane * 64u, sw = ((uint32_t)lane >> 1) & 3u;
-  if (lane == 0) bulk_wait_read0();
   __syncwarp();
 #pragma unroll
-  for (uint32_t j = 0; j < 4; ++j) sts_v4(row + ((j ^ sw) << 4), lw[4 * j], lw[4 * j + 1], lw[4 * j + 2], lw[4 * j + 3]);
+  for (uint32_t j = 0; j < 4; ++j) sts_v4(slab_lo + roff + ((j ^ sw) << 4), lw[4 * j], lw[4 * j + 1], lw[4 * j + 2], lw[4 * j + 3]);
   fence_async_smem();
   __syncwarp();
   if (lane == 0) {
-    tma_store_3d(o_lo, slab, cbase & 63, mrow0, cbase >> 6);
+    tma_store_3d(o_lo, slab_lo, cbase & 63, mrow0, cbase >> 6);
     bulk_commit();
   }
 }
@@ -312,8 +315,9 @@ __device__ __forceinline__ void store_slice_tma_lo(const CUtensorMap* o_lo, uint
 // and hands its 32 columns of each plane to the slab + TMA store path (fp16) or writes them with direct 16 B stores
 // (TF32: 128 B per plane).  ~10 instructions per element against ~29 of the staged path.
 template <int FMT>
-__device__ __forceinline__ void emit_slice_fwd_planes(const GemmParams& g, float* a, int lane, int mrow0, int cbase,
-                                                      const CUtensorMap* o_hi, const CUtensorMap* o_lo, uint32_t slab) {
+__device__ __forceinline__ void emit_slice_fwd_planes(const GemmParams& g, float* a, uint32_t drop_step, int lane, int mrow0,
+                                                      int cbase, const CUtensorMap* o_hi, const CUtensorMap* o_lo,
+                                                      uint32_t slab_hi, uint32_t slab_lo) {
   const int my_row = mrow0 + lane;
   const int kbo = cbase >> 5;
   if (kbo >= g.out_nb32) return;                         // warp-uniform
@@ -325,7 +329,7 @@ __device__ __forceinline__ void emit_slice_fwd_planes(const GemmParams& g, float
   if (g.drop_thresh != 0u) {
     // tf.layers.dropout in TRAIN mode (simple_dnn.py:80-81): x * 1/(1-rate) * keep; the mask is the counter-based hash
     // the oracle restates (oracle/adanet_oracle.py dropout_keep_mask): element index = row * out + col
-    const uint32_t key = g.drop_key0 + (uint32_t)(*g.drop_step) * 0xC2B2AE3Du;
+    const uint32_t key = g.drop_key0 + drop_step * 0xC2B2AE3Du;
     const uint32_t base = (uint32_t)my_row * (uint32_t)g.N + (uint32_t)cbase;
 #pragma unroll
     for (int j = 0; j < 32; ++j) {
@@ -339,15 +343,26 @@ __device__ __forceinline__ void emit_slice_fwd_planes(const GemmParams& g, float
     for (int j = 0; j < 32; ++j)
       if (!((cmask >> j) & 1u)) a[j] = 0.f;
   }
-  const bool tma = FMT == FMT_F16 && g.out_tma;
-  uint32_t lw[16];
-  if (tma) store_slice_tma_hi(o_hi, slab, a, lane, mrow0, cbase, lw);
-  uint32_t bits = 0u;               // (the sign bits are formed while the TMA unit reads the hi slab)
+  if (FMT == FMT_F16 && g.out_tma) store_slice_tma(o_hi, o_lo, slab_hi, slab_lo, a, lane, mrow0, cbase);
+  else if (my_row < g.M) store_row32_planes<FMT>(g, a, my_row, cbase);
+  uint32_t bits = 0u;
 #pragma unroll
   for (int j = 0; j < 32; ++j) bits |= (a[j] > 0.f) ? (1u << j) : 0u;
   if (my_row < g.M) g.out_bits[(size_t)kbo * g.M + my_row] = bits;
-  if (tma) store_slice_tma_lo(o_lo, slab, lw, lane, mrow0, cbase);
-  else if (my_row < g.M) store_row32_planes<FMT>(g, a, my_row, cbase);
+}
+
+// One round of the column-sum butterfly below, at distance W.  W is a template argument so that every index into `a`
+// is a constant: with the distance as a loop variable the inner loop stayed rolled, and `a` went to local memory.
+template <int W>
+__device__ __forceinline__ void colsum_round(float* a, int lane) {
+  const bool upper = (lane & W) != 0;
+#pragma unroll
+  for (int j = 0; j < W; ++j) {
+    const float x = a[j], y = a[j + W];
+    const float mine = upper ? y : x;
+    const float send = upper ? x : y;
+    a[j] = mine + __shfl_xor_sync(0xffffffffu, send, W);
+  }
 }
 
 // dX epilogue with planes out, without a register transpose: sign-bit ReLU mask, plane stores as in the forward
@@ -357,7 +372,8 @@ __device__ __forceinline__ void emit_slice_fwd_planes(const GemmParams& g, float
 // adds per lane, fixed order).
 template <int FMT>
 __device__ __forceinline__ void emit_slice_mask_planes(const GemmParams& g, float* a, uint32_t mwq, int lane, int mrow0, int cbase,
-                                                       const CUtensorMap* o_hi, const CUtensorMap* o_lo, uint32_t slab) {
+                                                       const CUtensorMap* o_hi, const CUtensorMap* o_lo, uint32_t slab_hi,
+                                                       uint32_t slab_lo) {
   const int my_row = mrow0 + lane;
   const int kbo = cbase >> 5;
   if (kbo >= g.out_nb32) return;                         // warp-uniform
@@ -372,38 +388,32 @@ __device__ __forceinline__ void emit_slice_mask_planes(const GemmParams& g, floa
     for (int j = 0; j < 32; ++j)
       if (!((keep >> j) & 1u)) a[j] = 0.f;
   }
-  const bool tma = FMT == FMT_F16 && g.out_tma;
-  uint32_t lw[16];
-  if (tma) store_slice_tma_hi(o_hi, slab, a, lane, mrow0, cbase, lw);
+  if (FMT == FMT_F16 && g.out_tma) store_slice_tma(o_hi, o_lo, slab_hi, slab_lo, a, lane, mrow0, cbase);
   else if (my_row < g.M) store_row32_planes<FMT>(g, a, my_row, cbase);
   if (g.colsum_part) {
-#pragma unroll
-    for (int w = 16; w >= 1; w >>= 1) {
-      const bool upper = (lane & w) != 0;
-#pragma unroll
-      for (int j = 0; j < w; ++j) {
-        const float mine = upper ? a[j + w] : a[j];
-        const float send = upper ? a[j] : a[j + w];
-        a[j] = mine + __shfl_xor_sync(0xffffffffu, send, w);
-      }
-    }
+    colsum_round<16>(a, lane);
+    colsum_round<8>(a, lane);
+    colsum_round<4>(a, lane);
+    colsum_round<2>(a, lane);
+    colsum_round<1>(a, lane);
     const int col = cbase + lane;
     if (col < g.colsum_ld) g.colsum_part[(size_t)(mrow0 >> 5) * g.colsum_ld + col] = a[0];
   }
-  if (tma) store_slice_tma_lo(o_lo, slab, lw, lane, mrow0, cbase);     // (after the column sums: they cover the hi store's read)
 }
 
 template <int FMT, int EPI>
 __device__ __forceinline__ void emit_slice(const GemmParams& g, const bool OUT_PLANES, float* a, uint32_t mwq, float* stage,
                                            int lane, int mrow0, int cbase, int rows_ok, float* dense, bool dense_vec,
                                            const bool bias_in_acc = false, const CUtensorMap* o_hi = nullptr,
-                                           const CUtensorMap* o_lo = nullptr) {
+                                           const CUtensorMap* o_lo = nullptr, uint32_t drop_step = 0u) {
+  // `stage` is the warp's hi slab; its lo' slab follows it
   if (EPI == EPI_BIAS_ACT && OUT_PLANES && bias_in_acc) {
-    emit_slice_fwd_planes<FMT>(g, a, lane, mrow0, cbase, o_hi, o_lo, smem_u32(stage));
+    emit_slice_fwd_planes<FMT>(g, a, drop_step, lane, mrow0, cbase, o_hi, o_lo, smem_u32(stage),
+                               smem_u32(stage + EPI_STAGE_FLOATS));
     return;
   }
   if (EPI == EPI_MASK && OUT_PLANES && bias_in_acc) {      // (the single-CTA kernel's direct path; out_mul is 1 for planes)
-    emit_slice_mask_planes<FMT>(g, a, mwq, lane, mrow0, cbase, o_hi, o_lo, smem_u32(stage));
+    emit_slice_mask_planes<FMT>(g, a, mwq, lane, mrow0, cbase, o_hi, o_lo, smem_u32(stage), smem_u32(stage + EPI_STAGE_FLOATS));
     return;
   }
   constexpr int SW = 16;                   // staged columns per pass (2 KB per warp, two passes)
@@ -577,6 +587,33 @@ __device__ __forceinline__ int find_problem(const Group& grp, int cur, int item,
 }
 __device__ __forceinline__ int first_next0(const Group& grp) { return grp.n > 1 ? grp.p[1].item0 : 0x7fffffff; }
 
+// One work item as the epilogue warpgroup sees it, with the global values its slices need: the ReLU-mask words of
+// the lane's row for the two 32-column halves (EPI_MASK; all ones without a mask, 0 past M or the last 32-column
+// block) and the dropout step (EPI_BIAS_ACT with dropout).
+struct EpiItem {
+  int p;                 // problem
+  Item it;
+  uint32_t mw0, mw1;
+  uint32_t drop_step;
+};
+template <int EPI>
+__device__ __forceinline__ EpiItem epi_fetch(const Group& grp, int& cur, int& next0, int item, int tile_row) {
+  EpiItem e;
+  cur = find_problem(grp, cur, item, next0);
+  e.p = cur;
+  const GemmParams& g = grp.p[cur].g;
+  e.it = decode_item(g, item - grp.p[cur].item0);
+  e.mw0 = e.mw1 = 0xffffffffu;
+  if (EPI == EPI_MASK && g.mask_bits) {
+    const int my_row = e.it.m0 + tile_row, kbo = e.it.n0 >> 5;
+    const bool row_ok = my_row < g.M;
+    e.mw0 = (row_ok && kbo < g.out_nb32) ? __ldg(g.mask_bits + (size_t)kbo * g.M + my_row) : 0u;
+    e.mw1 = (row_ok && kbo + 1 < g.out_nb32) ? __ldg(g.mask_bits + (size_t)(kbo + 1) * g.M + my_row) : 0u;
+  }
+  e.drop_step = (EPI == EPI_BIAS_ACT && g.drop_thresh != 0u) ? (uint32_t)(*g.drop_step) : 0u;
+  return e;
+}
+
 template <int R> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 template <int R> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 
@@ -741,24 +778,29 @@ pl_gemm_kernel(const __grid_constant__ Group grp) {
     // slices back row per lane and emits it; the staging tile is released once both slices are in registers.
     setmaxnreg_inc<EPI_REGS>();
     const int ew = warp - 4 * (1 + CONSUMERS);
-    float* stage = epi_stage + ew * EPI_STAGE_FLOATS;
+    float* stage = epi_stage + ew * 2 * EPI_STAGE_FLOATS;
+    const int row = 32 * ew + lane;
     int cur = 0, next0 = first_next0(grp);
+    // The global loads of a work item (mask words, dropout step) are issued one item ahead, before the wait for the
+    // current tile, so that they are not on the epilogue's critical path.
+    EpiItem nx{};
+    if ((int)blockIdx.x < n_items) nx = epi_fetch<EPI>(grp, cur, next0, blockIdx.x, row);
     uint32_t tcount = 0;
     for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++tcount) {
-      cur = find_problem(grp, cur, item, next0);
-      const GemmParams& g = grp.p[cur].g;
-      const Item it = decode_item(g, item - grp.p[cur].item0);
+      const EpiItem e = nx;
+      if (item + (int)gridDim.x < n_items) nx = epi_fetch<EPI>(grp, cur, next0, item + gridDim.x, row);
+      const GemmParams& g = grp.p[e.p].g;
+      const Item& it = e.it;
       const uint32_t buf = tcount & 1u;
       mbar_wait(smem_u32(&tile_full[buf]), (tcount >> 1) & 1u);
       const float* tile = acc_stage + buf * ACC_TILE_FLOATS;
-      const int row = 32 * ew + lane;
       const int mrow0 = it.m0 + 32 * ew;
-      const int my_row = mrow0 + lane;
       float* dense = reinterpret_cast<float*>(g.out);
       if (EPI == EPI_PARTIAL) dense += (size_t)it.split * g.M * g.N;
       const bool out_planes = g.out_planes != 0;
       const bool dense_vec = !out_planes && ((g.ldc & 3) == 0) && ((reinterpret_cast<uintptr_t>(dense) & 15) == 0);
       const int rows_ok = min(32, g.M - mrow0);          // warp-uniform; <= 0: nothing to write
+      const uint32_t mw0 = e.mw0, mw1 = e.mw1;
 #pragma unroll 1
       for (int h = 0; h < 2; ++h) {
         const int cs = 32 * h;
@@ -771,17 +813,13 @@ pl_gemm_kernel(const __grid_constant__ Group grp) {
         if (h == 1) mbar_arrive(smem_u32(&tile_empty[buf]));
         // ---- tile output: this warp's 32 rows x 32 columns ----
         const int ncol0 = it.n0 + cs;
-        uint32_t mw = 0xffffffffu;                     // ReLU mask: one sign-bit word per (row, 32-column block)
-        if (EPI == EPI_MASK && g.mask_bits) {
-          const int kbo = ncol0 >> 5;
-          mw = (my_row < g.M && kbo < g.out_nb32) ? __ldg(g.mask_bits + (size_t)kbo * g.M + my_row) : 0u;
-        }
-        if (FMT == FMT_F16) {     // the previous slice's TMA store must have read the staging slab
+        const uint32_t mw = h ? mw1 : mw0;
+        if (FMT == FMT_F16 && !out_planes) {     // the dense transpose reuses the hi slab: earlier TMA stores have read it
           if (lane == 0) bulk_wait_read0();
           __syncwarp();
         }
         emit_slice<FMT, EPI>(g, out_planes, acc, mw, stage, lane, mrow0, ncol0, rows_ok, dense, dense_vec, true,
-                             &grp.p[cur].o_hi, &grp.p[cur].o_lo);
+                             &grp.p[e.p].o_hi, &grp.p[e.p].o_lo, e.drop_step);
       }
     }
     if (FMT == FMT_F16 && lane == 0) bulk_wait0();    // stores complete before the CTA (and its shared memory) goes away
