@@ -602,74 +602,93 @@ int heads_group_init() {
 }
 }  // namespace adn
 
+namespace adn {
+// Checks op `idx` of adn_head_group and fills its launch parameters; touches no device memory.
+static int head_group_op(const adn_head_op& o, int idx, int64_t batch, int64_t dim, int fmt, int n_cta, HeadParams& p) {
+  if (!o.members_host || !o.out3 || !o.workspace) return fail(ADN_ERR_INVALID, "adn_head_group: op %d: null pointer", idx);
+  if (o.head < 0 || o.head > 2 || o.mixture_type < 0 || o.mixture_type > 2)
+    return fail(ADN_ERR_INVALID, "adn_head_group: op %d: bad head / mixture type", idx);
+  if (o.n_members < 1 || o.n_members > kMaxMembers)
+    return fail(ADN_ERR_UNSUPPORTED, "adn_head_group: op %d: n_members %d not in [1,%d]", idx, o.n_members, kMaxMembers);
+  if (o.mixture_type == ADN_MIX_MATRIX && o.dw) return fail(ADN_ERR_INVALID, "adn_head_group: op %d: dw must be NULL for MATRIX", idx);
+  if (!o.reg_is_zero && !o.gammas_host) return fail(ADN_ERR_INVALID, "adn_head_group: op %d: gammas missing", idx);
+  if (o.head == ADN_HEAD_SOFTMAX_XENT ? o.labels == nullptr : o.labels_f == nullptr)
+    return fail(ADN_ERR_INVALID, "adn_head_group: op %d: labels missing", idx);
+  if (o.dz_log2_scale < -60 || o.dz_log2_scale > 60) return fail(ADN_ERR_INVALID, "adn_head_group: op %d: bad dz_log2_scale", idx);
+  for (int k = 0; k < o.n_members; ++k) {
+    if (!o.members_host[k]) return fail(ADN_ERR_INVALID, "adn_head_group: op %d: member %d is null", idx, k);
+    p.members[k] = o.members_host[k];
+    p.gammas[k] = o.gammas_host ? o.gammas_host[k] : 0.f;
+  }
+  p.n_members = o.n_members;
+  p.head = o.head;
+  p.mixture = o.mixture_type;
+  p.w = o.w;
+  p.bias = o.bias;
+  p.labels = o.labels;
+  p.labels_f = o.labels_f;
+  p.dens = o.dens;
+  p.ens_out = o.ens_out;
+  if (o.dens_planes) {
+    p.densp = pl::plane_view(fmt, o.dens_planes, batch, dim);
+    p.dens_scale = ldexpf(1.0f, o.dz_log2_scale);
+    p.dens_nkb = (int)ceil_div(dim, pl::fmt_bk(fmt));
+    p.ovf = pl::overflow_flag();
+  }
+  p.batch = batch;
+  p.dim = (int)dim;
+  p.colsum_only = o.colsum_only ? 1 : 0;
+  p.want_grads = (o.dw || o.dbias) ? 1 : 0;
+  p.reg_is_zero = o.colsum_only ? 1 : o.reg_is_zero;
+  p.reg_multiplier = o.reg_multiplier;
+  p.out3 = o.out3;
+  p.dw = o.colsum_only ? nullptr : o.dw;
+  p.dbias = o.dbias;
+  const int wdim = (p.mixture == ADN_MIX_SCALAR) ? 1 : p.dim;
+  p.n_out = 1 + p.dim + p.n_members * wdim;
+  if (o.workspace_bytes < head_workspace_bytes(batch, dim, o.n_members))
+    return fail(ADN_ERR_WORKSPACE, "adn_head_group: op %d: workspace %lld < %lld bytes", idx, (long long)o.workspace_bytes,
+                (long long)head_workspace_bytes(batch, dim, o.n_members));
+  p.part = reinterpret_cast<float*>(o.workspace);
+  p.n_cta = n_cta;
+  return ADN_OK;
+}
+
+// Fills the launch of ops [i0, i0 + g.n) and the shared memory it needs.
+static int head_group_chunk(const adn_head_op* ops, int i0, int m, int64_t batch, int64_t dim, int fmt, int n_cta,
+                            HeadGroup& g, size_t& smem) {
+  g = HeadGroup{};
+  g.n = m;
+  smem = 0;
+  for (int i = 0; i < m; ++i) {
+    const int rc = head_group_op(ops[i0 + i], i0 + i, batch, dim, fmt, n_cta, g.p[i]);
+    if (rc) return rc;
+    smem = std::max(smem, head_smem_bytes(g.p[i].dim, g.p[i].n_members));
+  }
+  if (smem > 227 * 1024) return fail(ADN_ERR_UNSUPPORTED, "adn_head_group: members x dim does not fit shared memory");
+  return ADN_OK;
+}
+}  // namespace adn
+
 extern "C" int adn_head_group(const adn_head_op* ops, int n, int64_t batch, int64_t dim, void* stream) {
   if (n < 0 || (n > 0 && !ops)) return fail(ADN_ERR_INVALID, "adn_head_group: bad ops");
   if (batch <= 0 || dim <= 0 || dim > kMaxDim) return fail(ADN_ERR_INVALID, "adn_head_group: bad batch/dim");
   const int n_cta = (int)ceil_div(batch, kRows);
   const int fmt = pl::format();
+  const bool single_path = n_cta > 512;      // very large batches: two-level finalize of the single-head path
+  HeadGroup g;
+  size_t smem;
+  int rc;
+  // every op is checked before the first launch, so a rejected call writes nothing
+  for (int i0 = 0; i0 < n; i0 += kMaxGroup)
+    if ((rc = head_group_chunk(ops, i0, std::min(kMaxGroup, n - i0), batch, dim, fmt, n_cta, g, smem))) return rc;
   for (int i0 = 0; i0 < n; i0 += kMaxGroup) {
     const int m = std::min(kMaxGroup, n - i0);
-    HeadGroup g{};
-    g.n = m;
-    size_t smem = 0;
-    bool single_path = n_cta > 512;          // very large batches: two-level finalize of the single-head path
-    for (int i = 0; i < m; ++i) {
-      const adn_head_op& o = ops[i0 + i];
-      HeadParams& p = g.p[i];
-      if (!o.members_host || !o.out3 || !o.workspace) return fail(ADN_ERR_INVALID, "adn_head_group: op %d: null pointer", i0 + i);
-      if (o.head < 0 || o.head > 2 || o.mixture_type < 0 || o.mixture_type > 2)
-        return fail(ADN_ERR_INVALID, "adn_head_group: op %d: bad head / mixture type", i0 + i);
-      if (o.n_members < 1 || o.n_members > kMaxMembers)
-        return fail(ADN_ERR_UNSUPPORTED, "adn_head_group: op %d: n_members %d not in [1,%d]", i0 + i, o.n_members, kMaxMembers);
-      if (o.mixture_type == ADN_MIX_MATRIX && o.dw) return fail(ADN_ERR_INVALID, "adn_head_group: op %d: dw must be NULL for MATRIX", i0 + i);
-      if (!o.reg_is_zero && !o.gammas_host) return fail(ADN_ERR_INVALID, "adn_head_group: op %d: gammas missing", i0 + i);
-      if (o.head == ADN_HEAD_SOFTMAX_XENT ? o.labels == nullptr : o.labels_f == nullptr)
-        return fail(ADN_ERR_INVALID, "adn_head_group: op %d: labels missing", i0 + i);
-      if (o.dz_log2_scale < -60 || o.dz_log2_scale > 60) return fail(ADN_ERR_INVALID, "adn_head_group: op %d: bad dz_log2_scale", i0 + i);
-      for (int k = 0; k < o.n_members; ++k) {
-        if (!o.members_host[k]) return fail(ADN_ERR_INVALID, "adn_head_group: op %d: member %d is null", i0 + i, k);
-        p.members[k] = o.members_host[k];
-        p.gammas[k] = o.gammas_host ? o.gammas_host[k] : 0.f;
-      }
-      p.n_members = o.n_members;
-      p.head = o.head;
-      p.mixture = o.mixture_type;
-      p.w = o.w;
-      p.bias = o.bias;
-      p.labels = o.labels;
-      p.labels_f = o.labels_f;
-      p.dens = o.dens;
-      p.ens_out = o.ens_out;
-      if (o.dens_planes) {
-        p.densp = pl::plane_view(fmt, o.dens_planes, batch, dim);
-        p.dens_scale = ldexpf(1.0f, o.dz_log2_scale);
-        p.dens_nkb = (int)ceil_div(dim, pl::fmt_bk(fmt));
-        p.ovf = pl::overflow_flag();
-      }
-      p.batch = batch;
-      p.dim = (int)dim;
-      p.colsum_only = o.colsum_only ? 1 : 0;
-      p.want_grads = (o.dw || o.dbias) ? 1 : 0;
-      p.reg_is_zero = o.colsum_only ? 1 : o.reg_is_zero;
-      p.reg_multiplier = o.reg_multiplier;
-      p.out3 = o.out3;
-      p.dw = o.colsum_only ? nullptr : o.dw;
-      p.dbias = o.dbias;
-      const int wdim = (p.mixture == ADN_MIX_SCALAR) ? 1 : p.dim;
-      p.n_out = 1 + p.dim + p.n_members * wdim;
-      if (o.workspace_bytes < head_workspace_bytes(batch, dim, o.n_members))
-        return fail(ADN_ERR_WORKSPACE, "adn_head_group: op %d: workspace %lld < %lld bytes", i0 + i, (long long)o.workspace_bytes,
-                    (long long)head_workspace_bytes(batch, dim, o.n_members));
-      p.part = reinterpret_cast<float*>(o.workspace);
-      p.n_cta = n_cta;
-      smem = std::max(smem, head_smem_bytes(p.dim, p.n_members));
-    }
-    if (smem > 227 * 1024) return fail(ADN_ERR_UNSUPPORTED, "adn_head_group: members x dim does not fit shared memory");
+    if ((rc = head_group_chunk(ops, i0, m, batch, dim, fmt, n_cta, g, smem))) return rc;
     if (single_path) {
       for (int i = 0; i < m; ++i) {
         const adn_head_op& o = ops[i0 + i];
-        int rc = run_head(g.p[i], o.workspace, o.workspace_bytes, as_stream(stream));
-        if (rc) return rc;
+        if ((rc = run_head(g.p[i], o.workspace, o.workspace_bytes, as_stream(stream)))) return rc;
       }
       continue;
     }
@@ -692,14 +711,18 @@ extern "C" int adn_head_group(const adn_head_op* ops, int n, int64_t batch, int6
 
 extern "C" int adn_head_bookkeeping(const adn_head_book* books, int n, const int64_t* step_dev, void* stream) {
   if (n < 0 || (n > 0 && !books) || !step_dev) return fail(ADN_ERR_INVALID, "adn_head_bookkeeping: bad argument");
+  // every entry is checked before the first launch, so a rejected call writes nothing
+  for (int i = 0; i < n; ++i) {
+    const adn_head_book& b = books[i];
+    if (!b.ema_state || !b.out3 || !b.sub_loss || !b.trace || b.capacity < 1)
+      return fail(ADN_ERR_INVALID, "adn_head_bookkeeping: entry %d: bad argument", i);
+  }
   for (int i0 = 0; i0 < n; i0 += 64) {
     const int m = std::min(64, n - i0);
     BookGroup g{};
     g.n = m;
     for (int i = 0; i < m; ++i) {
       const adn_head_book& b = books[i0 + i];
-      if (!b.ema_state || !b.out3 || !b.sub_loss || !b.trace || b.capacity < 1)
-        return fail(ADN_ERR_INVALID, "adn_head_bookkeeping: entry %d: bad argument", i0 + i);
       g.e[i] = BookEntry{b.ema_state, b.out3, b.sub_loss, b.trace, b.decay, b.capacity};
     }
     head_bookkeeping_kernel<<<1, 64, 0, as_stream(stream)>>>(g, step_dev);

@@ -201,14 +201,18 @@ extern "C" int adn_opt_step(int kind, float* const* params_host, const float* co
 }
 
 namespace adn {
-// appends one optimizer's tensors to the launch description; returns 0 or an error
-static int add_optimizer(OptParams& o, StepPtrs& steps, int& chunks, int q, const adn_opt_op& op, const char* what) {
+static int n_slots(int kind) {
+  return kind == ADN_OPT_SGD ? 0 : ((kind == ADN_OPT_MOMENTUM || kind == ADN_OPT_MOMENTUM_COSINE) ? 1 : 2);
+}
+
+// checks one optimizer of a call; returns 0 or an error
+static int check_optimizer(const adn_opt_op& op, const char* what) {
   const int kind = op.kind;
   if (kind < ADN_OPT_SGD || kind > ADN_OPT_MOMENTUM_COSINE) return fail(ADN_ERR_INVALID, "%s: bad kind %d", what, kind);
   if (op.n_tensors < 1 || op.n_tensors > kMaxTensors)
     return fail(ADN_ERR_UNSUPPORTED, "%s: n_tensors %d not in [1,%d]", what, op.n_tensors, kMaxTensors);
   if (!op.params_host || !op.grads_host || !op.sizes_host || !op.hyper_host) return fail(ADN_ERR_INVALID, "%s: null pointer", what);
-  const int need_slots = kind == ADN_OPT_SGD ? 0 : ((kind == ADN_OPT_MOMENTUM || kind == ADN_OPT_MOMENTUM_COSINE) ? 1 : 2);
+  const int need_slots = n_slots(kind);
   if (need_slots >= 1 && !op.slot0_host) return fail(ADN_ERR_INVALID, "%s: slot0 required", what);
   if (need_slots >= 2 && !op.slot1_host) return fail(ADN_ERR_INVALID, "%s: slot1 required", what);
   if ((kind == ADN_OPT_ADAM || kind == ADN_OPT_MOMENTUM_COSINE) && !op.step_dev)
@@ -216,20 +220,30 @@ static int add_optimizer(OptParams& o, StepPtrs& steps, int& chunks, int q, cons
   if (kind == ADN_OPT_MOMENTUM_COSINE && !(op.hyper_host[2] > 0.f))
     return fail(ADN_ERR_INVALID, "%s: cosine decay needs decay_steps > 0", what);
   for (int i = 0; i < op.n_tensors; ++i) {
-    const int t = o.n;
     if (!op.params_host[i] || !op.grads_host[i] || op.sizes_host[i] <= 0)
       return fail(ADN_ERR_INVALID, "%s: tensor %d null or empty", what, i);
+    if ((need_slots >= 1 && !op.slot0_host[i]) || (need_slots >= 2 && !op.slot1_host[i]))
+      return fail(ADN_ERR_INVALID, "%s: slot for tensor %d is null", what, i);
+    if (op.planes_host && op.planes_host[i] &&
+        (!op.cols_host || op.cols_host[i] <= 0 || op.sizes_host[i] % op.cols_host[i] != 0 || op.cols_host[i] > INT32_MAX))
+      return fail(ADN_ERR_INVALID, "%s: tensor %d: cols must divide its size", what, i);
+  }
+  return ADN_OK;
+}
+
+// appends one checked optimizer's tensors to the launch description
+static void add_optimizer(OptParams& o, StepPtrs& steps, int& chunks, int q, const adn_opt_op& op) {
+  const int kind = op.kind;
+  const int need_slots = n_slots(kind);
+  for (int i = 0; i < op.n_tensors; ++i) {
+    const int t = o.n;
     o.p[t] = op.params_host[i];
     o.g[t] = op.grads_host[i];
     o.s0[t] = need_slots >= 1 ? op.slot0_host[i] : nullptr;
     o.s1[t] = need_slots >= 2 ? op.slot1_host[i] : nullptr;
-    if ((need_slots >= 1 && !o.s0[t]) || (need_slots >= 2 && !o.s1[t]))
-      return fail(ADN_ERR_INVALID, "%s: slot for tensor %d is null", what, i);
     o.size[t] = op.sizes_host[i];
     o.plane_hi[t] = nullptr;
     if (op.planes_host && op.planes_host[i]) {
-      if (!op.cols_host || op.cols_host[i] <= 0 || op.sizes_host[i] % op.cols_host[i] != 0 || op.cols_host[i] > INT32_MAX)
-        return fail(ADN_ERR_INVALID, "%s: tensor %d: cols must divide its size", what, i);
       const pl::PlaneView v = pl::plane_view(pl::format(), op.planes_host[i], op.sizes_host[i] / op.cols_host[i], op.cols_host[i]);
       o.plane_hi[t] = v.hi;
       o.plane_lo[t] = v.lo;
@@ -247,7 +261,6 @@ static int add_optimizer(OptParams& o, StepPtrs& steps, int& chunks, int q, cons
   o.h3[q] = kind >= ADN_OPT_RMSPROP ? op.hyper_host[3] : 0.f;   // MOMENTUM_COSINE (4): {lr, momentum, decay_steps, alpha}
   o.step_dev[q] = op.step_dev;
   if (op.step_dev) steps.p[steps.n++] = op.step_dev;
-  return ADN_OK;
 }
 
 static int flush(OptParams& o, StepPtrs& steps, int& chunks, cudaStream_t st) {
@@ -275,14 +288,20 @@ extern "C" int adn_opt_step_group(const adn_opt_op* ops, int n, void* stream) {
   o.n = 0;
   steps.n = 0;
   int chunks = 0, q = 0, rc;
+  // every op is checked before the first launch, so a rejected call changes no parameter, slot, plane or step counter
   for (int i = 0; i < n; ++i) {
     if (ops[i].n_tensors > kMaxTensors || ops[i].n_tensors < 1)
       return fail(ADN_ERR_UNSUPPORTED, "adn_opt_step_group: op %d: n_tensors %d not in [1,%d]", i, ops[i].n_tensors, kMaxTensors);
+    char what[48];
+    snprintf(what, sizeof(what), "adn_opt_step_group: op %d", i);
+    if ((rc = check_optimizer(ops[i], what))) return rc;
+  }
+  for (int i = 0; i < n; ++i) {
     if (o.n + ops[i].n_tensors > kMaxGroupTensors || q == kMaxGroupOpts) {
       if ((rc = flush(o, steps, chunks, as_stream(stream)))) return rc;
       q = 0;
     }
-    if ((rc = add_optimizer(o, steps, chunks, q, ops[i], "adn_opt_step_group"))) return rc;
+    add_optimizer(o, steps, chunks, q, ops[i]);
     ++q;
   }
   return flush(o, steps, chunks, as_stream(stream));

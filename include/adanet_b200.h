@@ -288,6 +288,7 @@ int adn_opt_step_p(int kind, float* const* params_host, const float* const* grad
  * adn_head_loss_p call (colsum_only = 1: members_host[0] = the logits, out3[0] = mean loss, dens / dens_planes =
  * dlogits dense / as planes times 2^dz_log2_scale, dbias = column sums of dlogits = the logits-layer bias gradient).
  * All ops share batch and dim.  workspace: adn_query(ADN_Q_HEAD_WORKSPACE_BYTES, batch, dim, n_members), one per op.
+ * Every op is checked before anything is launched: a call that returns an error has written nothing.
  */
 typedef struct adn_head_op {
   int32_t head;              /* ADN_HEAD_* */
@@ -315,7 +316,8 @@ typedef struct adn_head_op {
 } adn_head_op;
 int adn_head_group(const adn_head_op* ops_host, int n, int64_t batch, int64_t dim, void* stream);
 /* Per-step bookkeeping of n candidate ensembles in one launch: state <- zero-debiased EMA of out3[2] (adn_ema_update)
- * and trace[(*step_dev % capacity)][0..3] = {*sub_loss, out3[0], out3[2], ema} (adn_record_scalars). */
+ * and trace[(*step_dev % capacity)][0..3] = {*sub_loss, out3[0], out3[2], ema} (adn_record_scalars).  Every entry is
+ * checked before anything is launched: a call that returns an error has written nothing. */
 typedef struct adn_head_book {
   float* ema_state;
   const float* out3;
@@ -327,7 +329,9 @@ typedef struct adn_head_book {
 int adn_head_bookkeeping(const adn_head_book* books_host, int n, const int64_t* step_dev, void* stream);
 
 /* Grouped form of adn_opt_step_p: every optimizer of a training step (the subnetworks' and the mixture weights' of
- * every candidate on the GPU) in one launch.  Field meaning as the arguments of adn_opt_step_p. */
+ * every candidate on the GPU) in one launch.  Field meaning as the arguments of adn_opt_step_p.  Two ops of one call
+ * must not share a step_dev.  Every op is checked before anything is launched: a call that returns an error has
+ * changed no parameter, slot, plane or step counter. */
 typedef struct adn_opt_op {
   int32_t kind;
   int32_t n_tensors;
