@@ -20,7 +20,8 @@
 // Backward: dK[ky,kx,c,f] = sum_{b,p} patch(b, argmax(b,p,f))[ky,kx,c] * g[b,p,f], db[f] = sum g, where g is the
 // gradient w.r.t. the pooled features already masked by (pooled > 0) (the dX epilogue of the first dense layer
 // applies the sign bits written here).  One thread per (channel, filter) pair holding the nine taps, images looped
-// per CTA, per-CTA partials reduced in fixed order by a second kernel (deterministic).
+// per CTA, per-CTA partials reduced in fixed order by a second kernel (deterministic).  Images too large to stage
+// their gradient and arg-max words beside them take a variant that stages the image only.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -183,7 +184,10 @@ conv_stem_fwd_kernel(const float* __restrict__ images, const float* __restrict__
 // once per nine FMAs (the gather address depends on f through the arg-max, so taps are the only reuse there is).
 // G groups of CIN*F threads split the pooled pixels of an image; their accumulators are summed in fixed order
 // through shared memory once per CTA.
-template <int CIN, int F>
+// STAGE_G: g and the arg-max words are staged in shared memory with the image.  Large images do not fit that way;
+// the STAGE_G = false variant stages only the image and reads g / arg-max from global memory (read-only path).  The
+// arithmetic and its order are the same in both.
+template <int CIN, int F, bool STAGE_G>
 __global__ void __launch_bounds__(1024)
 conv_stem_bwd_kernel(const float* __restrict__ images, const uint32_t* __restrict__ argmax,
                      const float* __restrict__ dpooled, float* __restrict__ partials, int64_t B, int H, int W, int G) {
@@ -194,7 +198,7 @@ conv_stem_bwd_kernel(const float* __restrict__ images, const uint32_t* __restric
   const int prow = (W + 2) * CIN;
   // two staging sets {padded image, g [P*F], arg-max words [P*F/16]}: the next image is fetched under this one
   const int pimg4 = (pimg + 3) & ~3;
-  const int set_floats = pimg4 + P * F + ((P * F / 16 + 3) & ~3);     // 16-byte aligned sets
+  const int set_floats = STAGE_G ? pimg4 + P * F + ((P * F / 16 + 3) & ~3) : pimg4;     // 16-byte aligned sets
   float* s_set0 = smem;
   float* s_red = smem + 2 * set_floats;                           // [G][K*F + F]
   const int tid = threadIdx.x, nt = blockDim.x;
@@ -212,6 +216,7 @@ conv_stem_bwd_kernel(const float* __restrict__ images, const uint32_t* __restric
   const int64_t cols = (int64_t)P * F;
   auto stage = [&](float* set, int64_t bb) {
     stage_image<CIN>(set, images + bb * img_elems, H, W, tid, nt);
+    if (!STAGE_G) return;
     float* sg = set + pimg4;
     uint32_t* sa = reinterpret_cast<uint32_t*>(sg + P * F);
     for (int i = tid; i < (int)(cols / 4); i += nt) cp_async16(sg + 4 * i, dpooled + bb * cols + 4 * i);
@@ -228,16 +233,16 @@ conv_stem_bwd_kernel(const float* __restrict__ images, const uint32_t* __restric
     cp_async_wait<1>();
     __syncthreads();
     const float* s_img = s_set0 + buf * set_floats;
-    const float* s_g = s_img + pimg4;
-    const uint32_t* s_arg = reinterpret_cast<const uint32_t*>(s_g + P * F);
+    const float* g_img = STAGE_G ? s_img + pimg4 : dpooled + b * cols;
+    const uint32_t* a_img = STAGE_G ? reinterpret_cast<const uint32_t*>(s_img + pimg4 + P * F) : argmax + b * (cols / 16);
     // groups stride the pooled pixels of a row; tap addresses are three row pointers + compile-time offsets
     for (int py = 0; py < PH; ++py) {
-      const float* grow = s_g + (py * PW) * F + f;
-      const uint32_t* arow = s_arg + (py * PW) * fw + wsel;
+      const float* grow = g_img + (py * PW) * F + f;
+      const uint32_t* arow = a_img + (py * PW) * fw + wsel;
       const float* irow = s_img + (2 * py) * prow + c;
       for (int px = grp; px < PW; px += G) {
-        const float g = grow[px * F];
-        const uint32_t pos = (arow[px * fw] >> sh) & 3u;
+        const float g = STAGE_G ? grow[px * F] : __ldg(grow + px * F);
+        const uint32_t pos = ((STAGE_G ? arow[px * fw] : __ldg(arow + px * fw)) >> sh) & 3u;
         // padded coordinates of tap (0, 0) at the arg-max conv position (2py + dy, 2px + dx)
         const float* r0 = irow + (pos >> 1) * prow + (2 * px + (pos & 1u)) * CIN;
         const float* r1 = r0 + prow;
@@ -290,17 +295,24 @@ conv_stem_reduce_kernel(const float* __restrict__ partials, int n_part, int n_ou
 }
 
 static constexpr size_t kMaxSmem = 200 * 1024;
+// the image-only backward (STAGE_G = false): two padded images of up to 24 Ki floats plus the group partials need up to
+// 211,968 B, within the 232,448 B an H100 CTA may opt into
+static constexpr size_t kMaxSmemImageOnly = 227 * 1024;
 
 // Dynamic shared-memory limits are raised ONCE here (adn_init): cudaFuncSetAttribute inside a stream capture can
 // invalidate the capture (first use of a larger size while the engine records its CUDA graph).
 int init() {
-#define ADN_CONV_ATTR(K) ADN_CUDA(cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxSmem))
-  ADN_CONV_ATTR(conv_stem_fwd_kernel<1>);
-  ADN_CONV_ATTR(conv_stem_fwd_kernel<3>);
-  ADN_CONV_ATTR((conv_stem_bwd_kernel<1, 16>)); ADN_CONV_ATTR((conv_stem_bwd_kernel<3, 16>));
-  ADN_CONV_ATTR((conv_stem_bwd_kernel<1, 32>)); ADN_CONV_ATTR((conv_stem_bwd_kernel<3, 32>));
-  ADN_CONV_ATTR((conv_stem_bwd_kernel<1, 48>)); ADN_CONV_ATTR((conv_stem_bwd_kernel<3, 48>));
-  ADN_CONV_ATTR((conv_stem_bwd_kernel<1, 64>)); ADN_CONV_ATTR((conv_stem_bwd_kernel<3, 64>));
+#define ADN_CONV_ATTR(K, S) ADN_CUDA(cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(S)))
+#define ADN_CONV_BWD_ATTR(CIN, F)                                     \
+  ADN_CONV_ATTR((conv_stem_bwd_kernel<CIN, F, true>), kMaxSmem); \
+  ADN_CONV_ATTR((conv_stem_bwd_kernel<CIN, F, false>), kMaxSmemImageOnly)
+  ADN_CONV_ATTR(conv_stem_fwd_kernel<1>, kMaxSmem);
+  ADN_CONV_ATTR(conv_stem_fwd_kernel<3>, kMaxSmem);
+  ADN_CONV_BWD_ATTR(1, 16); ADN_CONV_BWD_ATTR(3, 16);
+  ADN_CONV_BWD_ATTR(1, 32); ADN_CONV_BWD_ATTR(3, 32);
+  ADN_CONV_BWD_ATTR(1, 48); ADN_CONV_BWD_ATTR(3, 48);
+  ADN_CONV_BWD_ATTR(1, 64); ADN_CONV_BWD_ATTR(3, 64);
+#undef ADN_CONV_BWD_ATTR
 #undef ADN_CONV_ATTR
   return ADN_OK;
 }
@@ -380,25 +392,36 @@ extern "C" int adn_conv_stem_bwd(const float* images, const uint32_t* argmax, co
   const int grid = conv::bwd_ctas(batch);
   const int pimg = (height + 2) * (width + 2) * channels;
   const int64_t cols = (int64_t)(height / 2) * (width / 2) * filters;
-  const size_t smem = (2 * ((size_t)((pimg + 3) & ~3) + cols + ((cols / 16 + 3) & ~(int64_t)3)) + (size_t)groups * (kf + filters)) * sizeof(float);
-  if (smem > conv::kMaxSmem) return fail(ADN_ERR_UNSUPPORTED, "adn_conv_stem_bwd: %zu bytes of staging do not fit", smem);
+  const size_t part_floats = (size_t)groups * (kf + filters);
+  const size_t img_floats = (size_t)((pimg + 3) & ~3);
+  const size_t smem_staged = (2 * (img_floats + cols + ((cols / 16 + 3) & ~(int64_t)3)) + part_floats) * sizeof(float);
+  const size_t smem_image = (2 * img_floats + part_floats) * sizeof(float);
+  // g and the arg-max words are staged with the image where they fit; otherwise only the image is (every shape
+  // check_shape accepts fits that way)
+  const bool staged = smem_staged <= conv::kMaxSmem;
+  const size_t smem = staged ? smem_staged : smem_image;
+  if (!staged && smem > conv::kMaxSmemImageOnly)
+    return fail(ADN_ERR_UNSUPPORTED, "adn_conv_stem_bwd: %zu bytes of staging do not fit", smem);
   float* partials = static_cast<float*>(workspace);
-  auto launch = [&](auto kern) -> int {
-    kern<<<grid, threads, smem, as_stream(stream)>>>(images, argmax, dpooled, partials, batch, height, width, groups);
+  auto launch = [&](auto kern_staged, auto kern_image) -> int {
+    if (staged) kern_staged<<<grid, threads, smem, as_stream(stream)>>>(images, argmax, dpooled, partials, batch, height, width, groups);
+    else kern_image<<<grid, threads, smem, as_stream(stream)>>>(images, argmax, dpooled, partials, batch, height, width, groups);
     ADN_CHECK_LAUNCH("conv_stem_bwd");
     return ADN_OK;
   };
+#define ADN_CONV_BWD(CIN, F) launch(conv::conv_stem_bwd_kernel<CIN, F, true>, conv::conv_stem_bwd_kernel<CIN, F, false>)
   int rc = ADN_OK;
   switch (filters / 16 * 4 + channels) {      // filters in {16,32,48,64} x channels in {1,3}
-    case 1 * 4 + 1: rc = launch(conv::conv_stem_bwd_kernel<1, 16>); break;
-    case 1 * 4 + 3: rc = launch(conv::conv_stem_bwd_kernel<3, 16>); break;
-    case 2 * 4 + 1: rc = launch(conv::conv_stem_bwd_kernel<1, 32>); break;
-    case 2 * 4 + 3: rc = launch(conv::conv_stem_bwd_kernel<3, 32>); break;
-    case 3 * 4 + 1: rc = launch(conv::conv_stem_bwd_kernel<1, 48>); break;
-    case 3 * 4 + 3: rc = launch(conv::conv_stem_bwd_kernel<3, 48>); break;
-    case 4 * 4 + 1: rc = launch(conv::conv_stem_bwd_kernel<1, 64>); break;
-    default: rc = launch(conv::conv_stem_bwd_kernel<3, 64>); break;
+    case 1 * 4 + 1: rc = ADN_CONV_BWD(1, 16); break;
+    case 1 * 4 + 3: rc = ADN_CONV_BWD(3, 16); break;
+    case 2 * 4 + 1: rc = ADN_CONV_BWD(1, 32); break;
+    case 2 * 4 + 3: rc = ADN_CONV_BWD(3, 32); break;
+    case 3 * 4 + 1: rc = ADN_CONV_BWD(1, 48); break;
+    case 3 * 4 + 3: rc = ADN_CONV_BWD(3, 48); break;
+    case 4 * 4 + 1: rc = ADN_CONV_BWD(1, 64); break;
+    default: rc = ADN_CONV_BWD(3, 64); break;
   }
+#undef ADN_CONV_BWD
   if (rc) return rc;
   const int n_out = kf + filters;
   conv::conv_stem_reduce_kernel<<<(n_out * 32 + 255) / 256, 256, 0, as_stream(stream)>>>(partials, grid, n_out, kf, dkernel,

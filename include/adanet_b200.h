@@ -367,7 +367,8 @@ int adn_l1_grad_add(float* dw, const float* w, int64_t n, float coef, void* stre
  * (pooled > 0) -- adn_dense_bwd_p(..., dx=dense, x_relu_mask=1) of the first dense layer produces exactly
  * that -- and returns dkernel [3,3,channels,filters] and dbias [filters] (fixed-order reduction).  No gradient
  * w.r.t. the images is formed (the stem is the first layer).
- * height, width even; channels in {1, 3}; filters in {16, 32, 48, 64}.
+ * height, width even; channels in {1, 3}; filters in {16, 32, 48, 64}; (height + 2) * (width + 2) * channels
+ * <= 24576.  Every shape the forward accepts, the backward accepts too.
  * workspace: adn_query(ADN_Q_CONV_STEM_BWD_WORKSPACE_BYTES, batch, channels, filters).
  */
 int adn_conv_stem_fwd(const float* images, const float* kernel, const float* bias, void* out_planes,
