@@ -56,9 +56,6 @@ static bool use_tc_bwd() {
 static constexpr int FWD_THREADS = 256;
 static constexpr int FC = 16;   // filters per accumulator chunk
 
-__device__ __forceinline__ float rna_tf32(float v) {
-  return __uint_as_float((__float_as_uint(v) + 0x1000u) & 0xffffe000u);
-}
 __device__ __forceinline__ void cp_async4(void* smem, const void* gmem) {
   const uint32_t s = (uint32_t)__cvta_generic_to_shared(smem);
   asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(s), "l"(gmem) : "memory");

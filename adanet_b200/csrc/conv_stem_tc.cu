@@ -30,9 +30,6 @@ static constexpr int THREADS = 256;
 static constexpr int TILE_BYTES = 128 * 128;   // one k-block (32 floats) of a 128-row K-major SWIZZLE_128B tile
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ float rna_tf32(float v) {
-  return __uint_as_float((__float_as_uint(v) + 0x1000u) & 0xffffe000u);
-}
 __device__ __forceinline__ void cp_async4(void* smem, const void* gmem) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_u32(smem)), "l"(gmem) : "memory");
 }
@@ -104,10 +101,11 @@ conv_stem_tc_fwd_kernel(const float* __restrict__ images, const float* __restric
     const int c = k % CIN, ij = k / CIN;
     const int ky = (ij >> 2) - (pos >> 1), kx = (ij & 3) - (pos & 1);
     const float v = (ky >= 0 && ky < 3 && kx >= 0 && kx < 3) ? kernel[((ky * 3 + kx) * CIN + c) * F + f] : 0.f;
-    const float h = rna_tf32(v);
+    float h, l;
+    pl::split_tf32(v, h, l);
     const uint32_t off = (uint32_t)(k >> 5) * NB + sw128(n, k & 31);
     *reinterpret_cast<float*>(s_w + off) = h;
-    *reinterpret_cast<float*>(s_w + KB * NB + off) = rna_tf32(v - h);
+    *reinterpret_cast<float*>(s_w + KB * NB + off) = l;
   }
   for (int i = tid; i < F; i += THREADS) s_b[i] = bias[i];
   for (int i = tid; i < NBUF * pimg; i += THREADS) s_img0[i] = 0.f;
@@ -153,10 +151,10 @@ conv_stem_tc_fwd_kernel(const float* __restrict__ images, const float* __restric
           const float2 v0 = *reinterpret_cast<const float2*>(patch + i * prow + o);        // 8-byte aligned (W even)
           const float2 v1 = *reinterpret_cast<const float2*>(patch + i * prow + o + 2);
           float4 h4, l4;
-          h4.x = rna_tf32(v0.x); l4.x = rna_tf32(v0.x - h4.x);
-          h4.y = rna_tf32(v0.y); l4.y = rna_tf32(v0.y - h4.y);
-          h4.z = rna_tf32(v1.x); l4.z = rna_tf32(v1.x - h4.z);
-          h4.w = rna_tf32(v1.y); l4.w = rna_tf32(v1.y - h4.w);
+          pl::split_tf32(v0.x, h4.x, l4.x);
+          pl::split_tf32(v0.y, h4.y, l4.y);
+          pl::split_tf32(v1.x, h4.z, l4.z);
+          pl::split_tf32(v1.y, h4.w, l4.w);
           const uint32_t off = (uint32_t)(q >> 3) * TILE_BYTES + rowoff + (uint32_t)((((q & 7) ^ (r & 7)) & 7) << 4);
           *reinterpret_cast<float4*>(a_hi + off) = h4;
           *reinterpret_cast<float4*>(a_lo + off) = l4;
@@ -311,10 +309,11 @@ conv_stem_tc_bwd_kernel(const float* __restrict__ images, const uint32_t* __rest
 #pragma unroll
           for (int e = 0; e < 4; ++e) {
             const int k = c4 * 4 + e;
-            const float h = rna_tf32(v[e]);
+            float h, l;
+            pl::split_tf32(v[e], h, l);
             const uint32_t off = kblk * (uint32_t)(K * 128) + sw128(k, col);
             *reinterpret_cast<float*>(at_hi + off) = h;
-            *reinterpret_cast<float*>(at_lo + off) = rna_tf32(v[e] - h);
+            *reinterpret_cast<float*>(at_lo + off) = l;
           }
         }
       } else {
@@ -338,8 +337,8 @@ conv_stem_tc_bwd_kernel(const float* __restrict__ images, const uint32_t* __rest
 #pragma unroll
           for (int e = 0; e < 16; ++e) {
             const uint32_t pos = (aw >> (2 * e)) & 3u;
-            const float h = rna_tf32(g[e]);
-            const float l = rna_tf32(g[e] - h);
+            float h, l;
+            pl::split_tf32(g[e], h, l);
             accb[f0 + e] += g[e];
 #pragma unroll
             for (int s = 0; s < 4; ++s) {

@@ -65,12 +65,20 @@ inline const uint32_t* bits_of(int fmt, const void* planes, int64_t rows, int64_
 }
 
 #ifdef __CUDACC__
-// hi = rna_tf32(v), lo = rna_tf32(v - hi).  cvt.rna.tf32.f32 is emulated in SASS; on the bit pattern it is "add
-// half a TF32 ulp to the magnitude, clear the low 13 bits" (Inf stays Inf, NaN stays NaN, finite values identical).
+// cvt.rna.tf32.f32 is emulated in SASS; on the bit pattern it is "add half a TF32 ulp to the magnitude, clear the low
+// 13 bits".  Finite values round as cvt.rna does (FLT_MAX and its neighbours round to Inf) and Inf stays Inf, but a NaN
+// whose top 11 mantissa bits are set carries through the exponent into the sign: the canonical NaN the GPU's own
+// arithmetic produces, 0x7FFFFFFF, becomes -0.  Only split_tf32 below may see a NaN.
 __device__ __forceinline__ float rna_tf32(float v) { return __uint_as_float((__float_as_uint(v) + 0x1000u) & 0xffffe000u); }
+// hi = rna_tf32(v), lo = rna_tf32(v - hi) for finite v; a NaN keeps its bits in hi and +-Inf is hi = +-Inf, lo = 0, so
+// that hi + lo is NaN / +-Inf again (rounding v - hi = NaN would make Inf's lo a NaN).
 __device__ __forceinline__ void split_tf32(float v, float& hi, float& lo) {
   hi = rna_tf32(v);
   lo = rna_tf32(v - hi);
+  if (!(fabsf(v) <= 3.402823466e38f)) {   // NaN or +-Inf: one compare with a free |.| modifier
+    hi = v;
+    lo = 0.f;
+  }
 }
 // hi = fp16(v), lo' = fp16((v - hi) * 2^11): v - hi is exact in fp32 (hi is v rounded to 11 bits)
 __device__ __forceinline__ void split_f16(float v, __half& hi, __half& lo) {

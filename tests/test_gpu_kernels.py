@@ -31,95 +31,6 @@ def _sp():
   return torch.cuda.current_stream().cuda_stream
 
 
-PATHS = ["simt", "auto"]
-
-
-def _set_path(name):
-  from adanet_b200 import _lib
-  _lib.set_dense_path({"simt": _lib.PATH_SIMT, "auto": _lib.PATH_AUTO, "tcgen05": _lib.PATH_TCGEN05}[name])
-
-
-# fp32 GEMM tolerance: |err| <= 2e-6 * sum_k |a||b| bound, checked as relative-to-max
-GEMM_RTOL = 3e-6
-
-
-@pytest.mark.parametrize("path", PATHS)
-@pytest.mark.parametrize("B,I,O,act", [
-    (256, 100, 64, 1), (1024, 100, 1024, 1), (512, 1024, 1024, 1), (300, 784, 128, 1), (1024, 1024, 10, 0),
-    (7, 5, 3, 0), (129, 33, 17, 1), (4096, 512, 512, 1), (128, 100, 10, 0),
-])
-def test_dense_fwd(gpu, path, B, I, O, act):
-  import torch
-  from adanet_b200 import _lib
-  _set_path(path)
-  rng = np.random.default_rng(B + I + O)
-  x = rng.standard_normal((B, I)).astype(np.float32)
-  w = orc.glorot_uniform(rng, I, O)
-  b = rng.standard_normal(O).astype(np.float32) * 0.1
-  want = x.astype(np.float64) @ w.astype(np.float64) + b
-  if act:
-    want = np.maximum(want, 0)
-  xd, wd, bd = _dev(x), _dev(w), _dev(b)
-  yd = torch.empty((B, O), dtype=torch.float32, device="cuda")
-  fws_bytes = _lib.query(_lib.Q_DENSE_FWD_WS, B, I, O)
-  fws = torch.empty((max(fws_bytes, 16),), dtype=torch.uint8, device="cuda")
-  _lib.check(gpu.adn_dense_fwd(xd.data_ptr(), wd.data_ptr(), bd.data_ptr(), yd.data_ptr(), B, I, O, act,
-                               fws.data_ptr(), fws_bytes, _sp()), "adn_dense_fwd")
-  got = yd.cpu().numpy()
-  scale = (np.abs(x).astype(np.float64) @ np.abs(w).astype(np.float64)).max()
-  assert np.abs(got - want).max() <= GEMM_RTOL * scale, (np.abs(got - want).max(), scale)
-  # no-bias variant
-  _lib.check(gpu.adn_dense_fwd(xd.data_ptr(), wd.data_ptr(), None, yd.data_ptr(), B, I, O, 0, fws.data_ptr(), fws_bytes,
-                               _sp()), "adn_dense_fwd")
-  want2 = x.astype(np.float64) @ w.astype(np.float64)
-  assert np.abs(yd.cpu().numpy() - want2).max() <= GEMM_RTOL * scale
-  _set_path("auto")
-
-
-@pytest.mark.parametrize("path", PATHS)
-@pytest.mark.parametrize("B,I,O,mask,want_dx", [
-    (256, 64, 10, 1, True), (1024, 1024, 1024, 1, True), (512, 100, 256, 0, False), (300, 128, 128, 1, True),
-    (4096, 512, 512, 1, True), (7, 5, 3, 0, True), (129, 33, 17, 1, True), (2048, 1024, 10, 1, True),
-])
-def test_dense_bwd(gpu, path, B, I, O, mask, want_dx):
-  import torch
-  from adanet_b200 import _lib
-  _set_path(path)
-  rng = np.random.default_rng(B * 3 + I + O)
-  x = rng.standard_normal((B, I)).astype(np.float32)
-  if mask:
-    x = np.maximum(x, 0)     # x is a ReLU output
-  w = orc.glorot_uniform(rng, I, O)
-  dz = (rng.standard_normal((B, O)) / B).astype(np.float32)
-  x64, w64, dz64 = x.astype(np.float64), w.astype(np.float64), dz.astype(np.float64)
-  want_dw = x64.T @ dz64
-  want_db = dz64.sum(0)
-  want_dxv = dz64 @ w64.T
-  if mask:
-    want_dxv = want_dxv * (x > 0)
-  ws_bytes = _lib.query(_lib.Q_DENSE_BWD_WS, B, I, O)
-  ws = torch.empty((ws_bytes,), dtype=torch.uint8, device="cuda")
-  xd, wd, dzd = _dev(x), _dev(w), _dev(dz)
-  dx = torch.full((B, I), 7.0, dtype=torch.float32, device="cuda") if want_dx else None
-  dw = torch.empty((I, O), dtype=torch.float32, device="cuda")
-  db = torch.empty((O,), dtype=torch.float32, device="cuda")
-  _lib.check(gpu.adn_dense_bwd(xd.data_ptr(), wd.data_ptr(), dzd.data_ptr(), dx.data_ptr() if want_dx else None,
-                               dw.data_ptr(), db.data_ptr(), B, I, O, mask, ws.data_ptr(), ws_bytes, _sp()),
-             "adn_dense_bwd")
-  s_dw = (np.abs(x64).T @ np.abs(dz64)).max()
-  assert np.abs(dw.cpu().numpy() - want_dw).max() <= GEMM_RTOL * s_dw
-  assert np.abs(db.cpu().numpy() - want_db).max() <= GEMM_RTOL * np.abs(dz64).sum(0).max()
-  if want_dx:
-    s_dx = (np.abs(dz64) @ np.abs(w64).T).max()
-    assert np.abs(dx.cpu().numpy() - want_dxv).max() <= GEMM_RTOL * s_dx
-  # determinism: a second launch gives bit-identical gradients
-  dw2 = torch.empty_like(dw)
-  _lib.check(gpu.adn_dense_bwd(xd.data_ptr(), wd.data_ptr(), dzd.data_ptr(), None, dw2.data_ptr(), db.data_ptr(),
-                               B, I, O, mask, ws.data_ptr(), ws_bytes, _sp()), "adn_dense_bwd")
-  assert torch.equal(dw, dw2)
-  _set_path("auto")
-
-
 @pytest.mark.parametrize("head,B,C", [(0, 256, 10), (0, 1000, 10), (0, 37, 3), (0, 4096, 16), (1, 300, 1), (2, 300, 1),
                                        (1, 128, 4), (0, 128, 64)])
 def test_head_loss(gpu, head, B, C):

@@ -196,17 +196,10 @@ def test_large_batch_dw_split_k(env):
   assert not _lib.plane_overflow()
 
 
-def test_colsum_and_opt_step_planes(env):
+def test_opt_step_planes(env):
   torch, _lib, lib = env
   rng = np.random.default_rng(5)
   sp = torch.cuda.current_stream().cuda_stream
-  a = rng.standard_normal((5000, 10)).astype(np.float32)
-  ad = torch.as_tensor(a).cuda()
-  out = torch.empty((10,), device="cuda")
-  nb = _lib.query(_lib.Q_COLSUM_WS, 5000, 10)
-  ws = torch.empty((nb,), dtype=torch.uint8, device="cuda")
-  _lib.check(lib.adn_colsum(ad.data_ptr(), 5000, 10, out.data_ptr(), ws.data_ptr(), nb, sp), "colsum")
-  assert _relerr(out.cpu().numpy(), a.astype(np.float64).sum(axis=0), np.abs(a).sum(axis=0).max()) < TOL
   # SGD step that refreshes the planes of a [100, 70] kernel; bias has no planes
   w = rng.standard_normal((100, 70)).astype(np.float32)
   g = rng.standard_normal((100, 70)).astype(np.float32)
