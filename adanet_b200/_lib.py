@@ -41,7 +41,7 @@ class FwdOp(ctypes.Structure):
   _fields_ = [("xp", c_void_p), ("wp", c_void_p), ("bias", c_void_p), ("yp", c_void_p), ("y", c_void_p),
               ("in_", c_int64), ("out", c_int64), ("act", ctypes.c_int32), ("reserved", ctypes.c_int32),
               ("dropout_rate", c_float), ("dropout_seed", ctypes.c_uint32), ("dropout_layer", ctypes.c_int32),
-              ("reserved2", ctypes.c_int32), ("dropout_step_dev", c_void_p)]
+              ("dropout_row0", ctypes.c_int32), ("dropout_step_dev", c_void_p)]
 
 
 class BwdOp(ctypes.Structure):

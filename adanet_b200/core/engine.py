@@ -408,10 +408,11 @@ class DenseNet:
                                             torch.cuda.current_stream(self.device).cuda_stream), "adn_planes_merge")
     return out
 
-  def fwd_op(self, i: int, xp: torch.Tensor, step_dev: Optional[torch.Tensor] = None) -> "_lib.FwdOp":
+  def fwd_op(self, i: int, xp: torch.Tensor, step_dev: Optional[torch.Tensor] = None, row0: int = 0) -> "_lib.FwdOp":
     """Layer i as an adn_fwd_op (plane path): hidden layers write planes, the logits layer dense fp32.  With
     `step_dev` (the plan's device step counter) the forward is the TRAIN-mode one: hidden layers with dropout draw
-    their keep mask for that step in the epilogue."""
+    their keep mask for that step in the epilogue -- for the rows row0, row0 + 1, ... of the minibatch when this net
+    trains a row slice of it."""
     last = i == len(self.ws) - 1
     src = (self.stem_out if self.stem else xp) if i == 0 else self.hp[i - 1]
     op = _lib.FwdOp(src.data_ptr(), self.wps[i].data_ptr(), self.bs[i].data_ptr(),
@@ -420,7 +421,7 @@ class DenseNet:
     d = self.dropout[i] if (self.dropout and step_dev is not None and not last and i < len(self.dropout)) else None
     if d is not None:
       op.dropout_rate, op.dropout_seed, op.dropout_layer = float(d[0]), int(d[1]) & 0xffffffff, i
-      op.dropout_step_dev = step_dev.data_ptr()
+      op.dropout_row0, op.dropout_step_dev = row0, step_dev.data_ptr()
     return op
 
   def dx_mul(self, i: int) -> float:
@@ -1136,11 +1137,12 @@ class IterationPlan:
         c.net.stem_forward(lib, x_of(c), sp)
     # layer waves: one grouped launch per wave and distinct batch size (whole candidates and frozen members run the
     # full minibatch, row-sharded candidates their slice)
-    fwd = ([(f, self.xp, self.batch, None) for f in self.frozen] +
-           [(c.net, xp_of(c), c.batch, self.step_dev) for c in self.candidates])       # candidates: TRAIN mode (dropout)
-    for w in range(max(len(n.ws) for n, _, _, _ in fwd)):
-      for bsz in sorted({b for _, _, b, _ in fwd}, reverse=True):
-        ops = [n.fwd_op(w, xp, sd) for n, xp, b, sd in fwd if b == bsz and w < len(n.ws)]
+    # candidates run in TRAIN mode (dropout); a row-sharded one draws its rows of the whole minibatch's mask
+    fwd = ([(f, self.xp, self.batch, None, 0) for f in self.frozen] +
+           [(c.net, xp_of(c), c.batch, self.step_dev, c.row0) for c in self.candidates])
+    for w in range(max(len(n.ws) for n, _, _, _, _ in fwd)):
+      for bsz in sorted({b for _, _, b, _, _ in fwd}, reverse=True):
+        ops = [n.fwd_op(w, xp, sd, r0) for n, xp, b, sd, r0 in fwd if b == bsz and w < len(n.ws)]
         if ops:
           _lib.check(lib.adn_dense_fwd_p_group((_lib.FwdOp * len(ops))(*ops), len(ops), bsz, sp), "adn_dense_fwd_p_group")
     # steps 3 and 6-11 of every candidate in one grouped launch (+ one finalize): the subnetwork losses (dlogits planes,
@@ -1323,10 +1325,14 @@ class IterationPlan:
     return [float(h.ema_state[2].item()) for _, h, _ in self.heads if self._reports(h)]
 
   def traces(self) -> Dict[str, Dict[str, np.ndarray]]:
+    """Per-step (sub_loss, ens_loss, adanet_loss, ema) of every head over the last min(steps_done, trace_capacity)
+    steps, oldest first.  Step s writes row s % trace_capacity of the ring, so once it has wrapped the oldest kept
+    step sits at row steps_done % trace_capacity."""
     n = min(self.steps_done, self.trace_capacity)
+    order = (np.arange(self.steps_done - n, self.steps_done) % self.trace_capacity) if n else np.zeros((0,), np.int64)
     out = {}
     for _, h, _ in self.heads:
-      t = h.trace[:n].cpu().numpy()
+      t = h.trace.cpu().numpy()[order]
       out[h.name] = {f: t[:, i].copy() for i, f in enumerate(TRACE_FIELDS)}
     return out
 

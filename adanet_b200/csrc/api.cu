@@ -237,6 +237,8 @@ extern "C" int adn_dense_fwd_p_group(const adn_fwd_op* ops, int n, int64_t batch
     if (ops[i].dropout_rate != 0.f) {
       if (!(ops[i].dropout_rate > 0.f && ops[i].dropout_rate < 1.f) || !ops[i].yp || !ops[i].dropout_step_dev)
         return fail(ADN_ERR_INVALID, "adn_dense_fwd_p_group: op %d: dropout needs 0 < rate < 1, planes out and a step counter", i);
+      if (ops[i].dropout_row0 < 0) return fail(ADN_ERR_INVALID, "adn_dense_fwd_p_group: op %d: dropout_row0 < 0", i);
+      o[i].dropout_row0 = ops[i].dropout_row0;
       o[i].dropout_rate = ops[i].dropout_rate;
       o[i].dropout_seed = ops[i].dropout_seed;
       o[i].dropout_layer = ops[i].dropout_layer;

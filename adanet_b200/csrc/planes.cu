@@ -125,6 +125,7 @@ struct GemmParams {
   uint32_t drop_thresh;  // keep iff hash >= thresh (= rate * 2^32)
   uint32_t drop_key0;    // seed * 0x9E3779B1 + layer * 0x85EBCA77 + 0x27D4EB2F  (the step term is added on the device)
   float drop_scale;      // 1 / (1 - rate)
+  uint32_t drop_idx0;    // element index of row 0 (row0 * N): a row slice of the minibatch draws the full batch's mask
   const int64_t* drop_step;
 };
 
@@ -328,9 +329,9 @@ __device__ __forceinline__ void emit_slice_fwd_planes(const GemmParams& g, float
   }
   if (g.drop_thresh != 0u) {
     // tf.layers.dropout in TRAIN mode (simple_dnn.py:80-81): x * 1/(1-rate) * keep; the mask is the counter-based hash
-    // the oracle restates (oracle/adanet_oracle.py dropout_keep_mask): element index = row * out + col
+    // the oracle restates (oracle/adanet_oracle.py dropout_keep_mask): element index = (row0 + row) * out + col
     const uint32_t key = g.drop_key0 + drop_step * 0xC2B2AE3Du;
-    const uint32_t base = (uint32_t)my_row * (uint32_t)g.N + (uint32_t)cbase;
+    const uint32_t base = g.drop_idx0 + (uint32_t)my_row * (uint32_t)g.N + (uint32_t)cbase;
 #pragma unroll
     for (int j = 0; j < 32; ++j) {
       uint32_t x = (base + (uint32_t)j) ^ key;
@@ -1293,6 +1294,7 @@ int dense_fwd_group(int fmt, const FwdOp* ops, int n, int64_t batch, cudaStream_
       if (g.drop_thresh == 0u) g.drop_thresh = 1u;
       g.drop_key0 = o.dropout_seed * 0x9E3779B1u + (uint32_t)o.dropout_layer * 0x85EBCA77u + 0x27D4EB2Fu;
       g.drop_scale = 1.0f / (1.0f - o.dropout_rate);
+      g.drop_idx0 = (uint32_t)((uint64_t)o.dropout_row0 * (uint64_t)o.out);
       g.drop_step = o.dropout_step;
     }
     if (o.yp) {

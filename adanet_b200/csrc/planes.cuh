@@ -28,6 +28,7 @@ struct FwdOp {
   float dropout_rate = 0.f;          // tf.layers.dropout on the output (planes out), see include/adanet_b200.h
   uint32_t dropout_seed = 0;
   int dropout_layer = 0;
+  int64_t dropout_row0 = 0;          // first minibatch row of a row slice: the mask is the full batch's
   const int64_t* dropout_step = nullptr;
 };
 struct BwdOp {

@@ -236,13 +236,15 @@ typedef struct adn_fwd_op {
   int32_t act;         /* ADN_ACT_* */
   int32_t reserved;
   /* tf.layers.dropout on the layer's output in TRAIN mode (adanet/examples/simple_dnn.py:80-81); planes out only.
-   * dropout_rate 0 = none.  keep iff hash32(seed, layer, *dropout_step_dev, row * out + col) >= rate * 2^32 (the mask
-   * is injected data shared with the oracle: oracle/adanet_oracle.py dropout_keep_mask), kept values are multiplied by
-   * 1 / (1 - rate), and the sign bits (= the backward mask) follow the dropped-out values. */
+   * dropout_rate 0 = none.  keep iff hash32(seed, layer, *dropout_step_dev, (dropout_row0 + row) * out + col) >=
+   * rate * 2^32 (the mask is injected data shared with the oracle: oracle/adanet_oracle.py dropout_keep_mask), kept
+   * values are multiplied by 1 / (1 - rate), and the sign bits (= the backward mask) follow the dropped-out values.
+   * dropout_row0 (>= 0, 0 = a whole minibatch): the first minibatch row of this op's rows when the op runs a row slice
+   * (a row-sharded candidate), so that every slice draws its rows of the whole minibatch's mask. */
   float dropout_rate;
   uint32_t dropout_seed;
   int32_t dropout_layer;
-  int32_t reserved2;
+  int32_t dropout_row0;
   const int64_t* dropout_step_dev;
 } adn_fwd_op;
 typedef struct adn_bwd_op {

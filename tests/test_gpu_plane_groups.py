@@ -389,21 +389,23 @@ def test_bwd_group_split_cap(env):
 
 
 def test_fwd_dropout_then_bwd_group(env):
-  """Two candidates' dropout forward (one group) feeding their backward (one group) with dx_mul = 1/(1-rate): dX is
-  (dz w^T) * keep * (relu > 0) / (1-rate), the mask read from the sign bits the forward wrote."""
+  """Three candidates' dropout forward (one group) feeding their backward (one group) with dx_mul = 1/(1-rate): dX is
+  (dz w^T) * keep * (relu > 0) / (1-rate), the mask read from the sign bits the forward wrote.  The third runs rows
+  1000..1999 of a minibatch (dropout_row0 = 1000, a row-sharded candidate): its mask is those rows of the whole
+  minibatch's mask, not the first 1000 rows'."""
   torch, _lib, lib = env
   from tests.parity_util import orc
   B, I, H, O, s = 1000, 100, 257, 65, 7
   rng = np.random.default_rng(41)
   step_dev = torch.full((), DROP_STEP, dtype=torch.int64, device="cuda")
   cands = []
-  for c, (seed, layer) in enumerate(((51, 1), (52, 2))):
+  for c, (seed, layer, row0) in enumerate(((51, 1, 0), (52, 2, 0), (51, 1, 1000))):
     x = _mag(rng, (B, I))
     w1 = (_mag(rng, (I, H)) / np.sqrt(I)).astype(np.float32)
     b1 = _mag(rng, (H,))
     w2 = (_mag(rng, (H, O)) / np.sqrt(O)).astype(np.float32)
     dz = (_mag(rng, (B, O)) * 2.0 ** -s).astype(np.float32)
-    cands.append(dict(seed=seed, layer=layer, x=x, w1=w1, b1=b1, w2=w2, dz=dz, xp=_planes(torch, _lib, lib, x),
+    cands.append(dict(seed=seed, layer=layer, row0=row0, x=x, w1=w1, b1=b1, w2=w2, dz=dz, xp=_planes(torch, _lib, lib, x),
                       w1p=_planes(torch, _lib, lib, w1), b1d=torch.as_tensor(b1).cuda(), w2p=_planes(torch, _lib, lib, w2),
                       dzp=_planes(torch, _lib, lib, dz, s),
                       hp=torch.zeros((_lib.query(_lib.Q_PLANES_BYTES, B, H) // 4,), device="cuda")))
@@ -411,9 +413,9 @@ def test_fwd_dropout_then_bwd_group(env):
   for c in cands:
     op = _lib.FwdOp(c["xp"].data_ptr(), c["w1p"].data_ptr(), c["b1d"].data_ptr(), c["hp"].data_ptr(), None, I, H, 1, 0)
     op.dropout_rate, op.dropout_seed, op.dropout_layer = DROP_RATE, c["seed"], c["layer"]
-    op.dropout_step_dev = step_dev.data_ptr()
+    op.dropout_row0, op.dropout_step_dev = c["row0"], step_dev.data_ptr()
     fops.append(op)
-  _lib.check(lib.adn_dense_fwd_p_group((_lib.FwdOp * 2)(*fops), 2, B, _stream(torch)), "adn_dense_fwd_p_group")
+  _lib.check(lib.adn_dense_fwd_p_group((_lib.FwdOp * 3)(*fops), 3, B, _stream(torch)), "adn_dense_fwd_p_group")
   bops, bufs = [], []
   for c in cands:
     d = dict(I=H, O=O, mask=1, s=s, mul=DX_MUL, outs={"dw", "dxp", "cs"}, x=None, dz=c["dz"], w=c["w2"], xp=c["hp"],
@@ -430,7 +432,7 @@ def test_fwd_dropout_then_bwd_group(env):
     pos = np.zeros((B, nb32 * 32), dtype=bool)
     pos[:, :H] = h > 0
     assert np.array_equal(bits, _bits_of(pos))
-    keep = orc.dropout_keep_mask(c["seed"], c["layer"], DROP_STEP, B, H, DROP_RATE)
+    keep = orc.dropout_keep_mask(c["seed"], c["layer"], DROP_STEP, c["row0"] + B, H, DROP_RATE)[c["row0"]:]
     x64, w164 = c["x"].astype(np.float64), c["w1"].astype(np.float64)
     relu = np.maximum(x64 @ w164 + c["b1"], 0.0)
     assert not (pos[:, :H] & ~keep).any()
