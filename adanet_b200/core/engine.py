@@ -53,12 +53,41 @@ TRACE_FIELDS = ("sub_loss", "ens_loss", "adanet_loss", "ema")
 EVAL_METRICS = ("adanet_loss", "loss", "average_loss", "accuracy")
 
 
-def accuracy_of(logits: torch.Tensor, labels: torch.Tensor) -> float:
-  """Fraction of examples whose predicted class equals the label: arg-max for [B, C>1] logits against int labels,
-  logit > 0 for a single-logit (sigmoid) head against {0,1} labels.  Evaluation bookkeeping, not on the step path."""
+def correct_of(logits: torch.Tensor, labels: torch.Tensor) -> Tuple[int, int]:
+  """(correct, total) predictions: arg-max for [B, C>1] logits against int labels, logit > 0 for a single-logit
+  (sigmoid) head against {0,1} labels.  Evaluation bookkeeping, not on the step path."""
   if logits.shape[1] > 1:
-    return float((logits.argmax(dim=1) == labels.reshape(-1)).float().mean().item())
-  return float(((logits.reshape(-1) > 0) == (labels.reshape(-1) > 0.5)).float().mean().item())
+    return int((logits.argmax(dim=1) == labels.reshape(-1)).sum().item()), int(logits.shape[0])
+  return int(((logits.reshape(-1) > 0) == (labels.reshape(-1) > 0.5)).sum().item()), int(logits.numel())
+
+
+def accuracy_of(logits: torch.Tensor, labels: torch.Tensor) -> float:
+  """Fraction of correct predictions (correct_of)."""
+  correct, total = correct_of(logits, labels)
+  return correct / total
+
+
+def _check_head_ws(rows: int, logits_dim: int, n_members: int, have: int):
+  """A head launched on the first `rows` examples of buffers sized for the static batch must fit the workspace
+  allocated for that batch."""
+  need = _lib.query(_lib.Q_HEAD_WS, rows, logits_dim, n_members)
+  if need > have:
+    raise RuntimeError("head workspace of %d bytes is too small for %d rows (needs %d)" % (have, rows, need))
+
+
+def _load_rows(x_buf: torch.Tensor, labels_buf: Optional[torch.Tensor], x, y) -> int:
+  """Copies an evaluation batch of b <= batch examples into the first b rows of the static-batch buffers and zeroes
+  the rest; returns b.  `y` may be None (predict): the labels buffer is then left alone."""
+  x = torch.as_tensor(x)
+  b, batch = int(x.shape[0]), int(x_buf.shape[0])
+  if not 0 < b <= batch:
+    raise ValueError("an evaluation batch of %d examples does not fit the static batch of %d" % (b, batch))
+  x_buf[:b].copy_(x.reshape((b,) + tuple(x_buf.shape[1:])), non_blocking=True)
+  x_buf[b:].zero_()
+  if y is not None:
+    labels_buf[:b].copy_(torch.as_tensor(y).reshape((b,) + tuple(labels_buf.shape[1:])), non_blocking=True)
+    labels_buf[b:].zero_()
+  return b
 
 
 def _stream_ptr(stream: Optional[torch.cuda.Stream] = None) -> int:
@@ -657,15 +686,19 @@ class EnsembleHead:
     if train_ens:
       self.ens_opt.apply(lib, self._ens_grads, sp)
 
-  def enqueue_eval(self, labels, labels_f, ens_out: Optional[torch.Tensor], sp: int, xp: Optional[torch.Tensor] = None):
-    """Forward-only ensemble logits / loss over the members' current logits (Evaluator, evaluate, predict)."""
+  def enqueue_eval(self, labels, labels_f, ens_out: Optional[torch.Tensor], sp: int, xp: Optional[torch.Tensor] = None,
+                   rows: Optional[int] = None):
+    """Forward-only ensemble logits / loss over the members' current logits (Evaluator, evaluate, predict), on the
+    first `rows` examples (default: the whole batch) -- row-major logits make them a prefix of every member's."""
+    rows = self.batch if rows is None else rows
+    _check_head_ws(rows, self.C, len(self.member_nets), self.head_ws_bytes)
     if self.mix == _lib.MIX_MATRIX:
       self.matrix_forward(xp, sp)
     _lib.check(self.lib.adn_ensemble_head(
         self.head, self.mix, self._members, len(self.member_nets), self.mix_w.data_ptr(), self.bias.data_ptr(),
         self._gammas, self.reg_is_zero, self.reg_multiplier,
         labels.data_ptr() if labels is not None else None, labels_f.data_ptr() if labels_f is not None else None,
-        self.out3.data_ptr(), None, None, None, ens_out.data_ptr() if ens_out is not None else None, self.batch,
+        self.out3.data_ptr(), None, None, None, ens_out.data_ptr() if ens_out is not None else None, rows,
         self.C, self.head_ws.data_ptr(), self.head_ws_bytes, sp), "adn_ensemble_head")
 
   def mixture_weight_tensors(self) -> List[torch.Tensor]:
@@ -1253,16 +1286,19 @@ class IterationPlan:
     self.steps_done += 1
 
   def eval_step(self, x, y, metric: str = "adanet_loss") -> List[float]:
-    """Forward-only metric of every local candidate ensemble on one hold-out batch (the Evaluator path,
-    adanet/core/estimator.py:1469-1490): "adanet_loss" (default), "loss" / "average_loss" (the head's mean loss) or
-    "accuracy" (classification heads; arg-max of the ensemble logits, sigmoid heads at 0)."""
+    """Forward-only metric of every local candidate ensemble on one hold-out batch of b <= batch examples (the
+    Evaluator path, adanet/core/estimator.py:1469-1490): "adanet_loss" (default), "loss" / "average_loss" (the
+    head's mean loss over the b examples) or "accuracy" (classification heads; arg-max of the ensemble logits,
+    sigmoid heads at 0).  The members run in inference mode (no dropout) at the static batch, a partial batch
+    zero-padded; the heads read the first b rows."""
     if metric not in EVAL_METRICS:
       raise NotImplementedError("Evaluator metric %r is not computed by the B200 engine (supported: %s)" % (metric, ", ".join(EVAL_METRICS)))
     if metric == "accuracy" and self.head == "mse":
       raise ValueError("accuracy is not an evaluation metric of a regression head")
     if self.sharded:
       raise NotImplementedError("hold-out evaluation of row-sharded candidates: use placement='balanced' with an Evaluator")
-    self.load_batch(x, y)
+    labels = self.labels if self.labels is not None else self.labels_f
+    b = _load_rows(self.x, labels, x, y)
     sp = torch.cuda.current_stream(self.device).cuda_stream
     self._split_x(sp)
     for f in self.frozen:
@@ -1272,9 +1308,9 @@ class IterationPlan:
     out = []
     ens_out = torch.empty((self.batch, self.C), dtype=torch.float32, device=self.device) if metric == "accuracy" else None
     for _, h, _ in self.heads:
-      h.enqueue_eval(self.labels, self.labels_f, ens_out, sp, self.xp)
+      h.enqueue_eval(self.labels, self.labels_f, ens_out, sp, self.xp, rows=b)
       if metric == "accuracy":
-        out.append(accuracy_of(ens_out, self.labels if self.labels is not None else self.labels_f))
+        out.append(accuracy_of(ens_out[:b], labels[:b]))
     torch.cuda.current_stream(self.device).synchronize()
     if metric == "accuracy":
       return out
@@ -1353,6 +1389,7 @@ class EnsembleEvalPlan:
     self.lib = _require_cuda()
     self.device = device or torch.device("cuda", torch.cuda.current_device())
     self.members, self.batch, self.C, self.head = list(members), batch, logits_dim, _HEAD_KIND[head]
+    self.fmt = _lib.plane_format()      # xp / mwp are sized for it: a plan outlives no format switch
     for m in self.members:
       m.ensure_format()
       if m.batch != batch:
@@ -1384,6 +1421,7 @@ class EnsembleEvalPlan:
                                    else [m.logits.data_ptr() for m in self.members])
     self.out3 = torch.zeros((3,), **f32)
     self.ens_logits = torch.empty((batch, logits_dim), **f32)
+    self.rows = 0             # examples of the last `run`: its logits are the first rows of ens_logits
     self.ws_bytes = _lib.query(_lib.Q_HEAD_WS, batch, logits_dim, len(self.members))
     self.workspace = torch.empty((self.ws_bytes,), dtype=torch.uint8, device=self.device)
     self.x = torch.empty((batch, members[0].in_dim), **f32)
@@ -1392,15 +1430,13 @@ class EnsembleEvalPlan:
     self.labels_f = torch.zeros((batch, logits_dim), **f32) if head != "softmax_xent" else None
 
   def run(self, x, y=None, forward_members: bool = True):
-    """Returns (loss, reg, adanet_loss) as floats (NaN-free only when labels given) and leaves
-    the ensemble logits in `self.ens_logits`."""
+    """Evaluates the ensemble on the b <= batch examples of `x`: returns (loss, reg, adanet_loss) over them as
+    floats (NaN-free only when labels given) and leaves their ensemble logits in the first b rows of
+    `self.ens_logits` (`self.rows` = b).  The members run at the static batch, a partial batch zero-padded."""
     sp = torch.cuda.current_stream(self.device).cuda_stream
-    self.x.copy_(torch.as_tensor(x).reshape(self.x.shape), non_blocking=True)
-    if y is not None:
-      if self.labels is not None:
-        self.labels.copy_(torch.as_tensor(y).reshape(self.batch), non_blocking=True)
-      else:
-        self.labels_f.copy_(torch.as_tensor(y).reshape(self.batch, self.C), non_blocking=True)
+    b = _load_rows(self.x, self.labels if self.labels is not None else self.labels_f, x, y)
+    self.rows = b
+    _check_head_ws(b, self.C, len(self.members), self.ws_bytes)
     if forward_members:
       if self.xp is not None and any(not m.stem for m in self.members):
         _lib.check(self.lib.adn_planes_split(self.x.data_ptr(), self.batch, self.x.shape[1], self.xp.data_ptr(), sp),
@@ -1416,7 +1452,7 @@ class EnsembleEvalPlan:
         self.head, self.mix, self._members, len(self.members), self.mix_w.data_ptr(), self.bias.data_ptr(),
         self._gammas, self.reg_is_zero, 1.0, self.labels.data_ptr() if self.labels is not None else None,
         self.labels_f.data_ptr() if self.labels_f is not None else None, self.out3.data_ptr(), None, None, None,
-        self.ens_logits.data_ptr(), self.batch, self.C, self.workspace.data_ptr(), self.ws_bytes, sp),
+        self.ens_logits.data_ptr(), b, self.C, self.workspace.data_ptr(), self.ws_bytes, sp),
                "adn_ensemble_head")
     o = self.out3.cpu().numpy()
     return float(o[0]), float(o[1]), float(o[2])
@@ -1429,5 +1465,6 @@ class EnsembleEvalPlan:
     if metric == "accuracy":
       if self.head == _lib.HEAD_MSE:
         raise ValueError("accuracy is not an evaluation metric of a regression head")
-      return accuracy_of(self.ens_logits, self.labels if self.labels is not None else self.labels_f)
+      b = self.rows
+      return accuracy_of(self.ens_logits[:b], (self.labels if self.labels is not None else self.labels_f)[:b])
     return adanet if metric == "adanet_loss" else loss

@@ -714,7 +714,10 @@ class Estimator(object):
     s = self._search
     if s is None or not s.frozen:
       raise ValueError("no trained ensemble yet: train at least one AdaNet iteration before evaluate/predict")
-    if self._eval_plan is None:
+    from adanet_b200 import _lib
+    if self._eval_plan is None or self._eval_plan.fmt != _lib.plane_format():
+      # built anew after the fp16 -> TF32 fallback too: its planes (and the members', EnsembleEvalPlan re-creates
+      # them) are sized by the format they were built in
       self._eval_plan = eng.EnsembleEvalPlan(s.frozen, s.mixture_weights, s.bias, s.winner_ens, s.head, s.batch, s.C, s.device)
     return self._eval_plan
 
@@ -723,47 +726,48 @@ class Estimator(object):
     return "| {} |".format(" | ".join(name for _, name in self._architecture.subnetworks))
 
   def evaluate(self, input_fn, steps=None, hooks=None, checkpoint_path=None, name=None):
-    """Mean loss of the best ensemble over `steps` batches (+ accuracy for classification),
-    `global_step`, `iteration` and the architecture string (eval_metrics.py:227-264,347-393)."""
+    """Metrics of the best ensemble over `steps` batches of at most the training batch size, a partial last batch
+    included: `loss` (the mean of the per-batch mean losses), `average_loss` (the mean over examples), `accuracy`
+    for classification heads (over examples), `global_step`, `iteration` and the architecture string
+    (eval_metrics.py:120,227-264,347-393)."""
+    import torch
+    from adanet_b200.core import engine as eng
     self._restore_for_inference(input_fn)
     plan = self._ensemble_eval_plan()
-    n, loss_sum, correct, total = 0, 0.0, 0, 0
+    n, loss_sum, examples, example_loss_sum, correct, total = 0, 0.0, 0, 0.0, 0, 0
     for features, labels in input_utils.iterate_input_fn(input_fn):
       if steps is not None and n >= steps:
         break
-      if input_utils.batch_size_of(features) != self._batch_size:
-        input_utils.warn_ragged(input_utils.batch_size_of(features), self._batch_size)
-        continue
       loss, _, _ = plan.run(input_utils.to_matrix(features, self._feature_keys), labels)
+      b = plan.rows
       loss_sum += loss
       n += 1
-      if self._head.loss_kind == "softmax_xent":
-        import torch
-        pred = plan.ens_logits.argmax(dim=1).cpu()
-        lab = torch.as_tensor(labels).reshape(-1).cpu()
-        correct += int((pred == lab).sum())
-        total += int(lab.numel())
+      example_loss_sum += loss * b
+      examples += b
+      if self._head.loss_kind != "mse":
+        c, t = eng.correct_of(plan.ens_logits[:b], torch.as_tensor(labels).to(plan.device))
+        correct += c
+        total += t
     if n == 0:
-      raise ValueError("evaluate: input_fn produced no full batches")
-    out = {"loss": loss_sum / n, "average_loss": loss_sum / n, "global_step": self._global_step,
+      raise ValueError("evaluate: input_fn produced no batches")
+    out = {"loss": loss_sum / n, "average_loss": example_loss_sum / examples, "global_step": self._global_step,
            "iteration": self._search.iteration, "architecture/adanet/ensembles": self.architecture_string()}
     if total:
       out["accuracy"] = correct / total
     return out
 
   def predict(self, input_fn, predict_keys=None, hooks=None, checkpoint_path=None, yield_single_examples=True):
-    """Yields per-example predictions of the best ensemble: logits (+ probabilities / class_ids
-    for MultiClassHead, logistic for BinaryClassHead, predictions for RegressionHead)."""
+    """Yields per-example predictions of the best ensemble, one per input example (batches of at most the training
+    batch size, a partial last batch included): logits (+ probabilities / class_ids for MultiClassHead, logistic for
+    BinaryClassHead, predictions for RegressionHead)."""
     import torch
     self._restore_for_inference(input_fn)
     plan = self._ensemble_eval_plan()
     for item in input_utils.iterate_input_fn(input_fn):
       features = item[0] if isinstance(item, tuple) else item
-      if input_utils.batch_size_of(features) != self._batch_size:
-        input_utils.warn_ragged(input_utils.batch_size_of(features), self._batch_size)
-        continue
       plan.run(input_utils.to_matrix(features, self._feature_keys), None)
-      logits = plan.ens_logits
+      b = plan.rows
+      logits = plan.ens_logits[:b]
       out = {"logits": logits.cpu().numpy()}
       if self._head.loss_kind == "softmax_xent":
         out["probabilities"] = torch.softmax(logits, dim=1).cpu().numpy()
@@ -775,7 +779,7 @@ class Estimator(object):
       if predict_keys:
         out = {k: v for k, v in out.items() if k in predict_keys}
       if yield_single_examples:
-        for i in range(self._batch_size):
+        for i in range(b):
           yield {k: v[i] for k, v in out.items()}
       else:
         yield out

@@ -42,15 +42,20 @@ class Evaluator(object):
   def evaluate(self, evaluate_batch_fn, num_candidates):
     """Streams up to `steps` batches of `input_fn` through `evaluate_batch_fn(features, labels)`
     (which returns one metric value per candidate for that batch) and returns the per-candidate
-    mean, like the tf.metrics.mean accumulators of evaluator.py:97-140."""
-    from adanet_b200.core.input_utils import iterate_input_fn
+    mean, like the tf.metrics.mean accumulators of evaluator.py:97-140: "adanet_loss" and "loss" are
+    per-batch scalars, weighted per batch (eval_metrics.py:120); "average_loss" and "accuracy" are
+    weighted by the batch's example count, so a partial last batch counts for its examples."""
+    from adanet_b200.core.input_utils import batch_size_of, iterate_input_fn
+    per_example = self._metric_name in ("average_loss", "accuracy")
     sums = np.zeros((num_candidates,), dtype=np.float64)
-    n = 0
+    n, weight = 0, 0.0
     for features, labels in iterate_input_fn(self._input_fn):
       if self._steps is not None and n == self._steps:
         break
-      sums += np.asarray(evaluate_batch_fn(features, labels), dtype=np.float64)
+      w = float(batch_size_of(features)) if per_example else 1.0
+      sums += w * np.asarray(evaluate_batch_fn(features, labels), dtype=np.float64)
       n += 1
+      weight += w
     if n == 0:
       raise ValueError("Evaluator input_fn produced no batches")
-    return list(sums / n)
+    return list(sums / weight)

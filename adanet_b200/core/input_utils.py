@@ -5,8 +5,9 @@ The reference's `input_fn` returns TF tensors / a tf.data.Dataset.  Here an
 `(features, labels)` minibatches, where `features` is an array [B, D] or a dict
 of column key -> array [B, d_k] (NumPy or torch, host or device) and `labels`
 an array [B] / [B, 1] (class ids) or [B, C] (regression / binary targets).
-Every batch must have the same size (a static-shape engine: ragged tails are
-dropped with a warning, cf. `drop_remainder`).
+Training batches must all have the same size (a static-shape engine: ragged
+tails are dropped with a warning, cf. `drop_remainder`).  Evaluation and
+prediction take batches of up to that size, so a partial last batch counts.
 """
 
 import logging
