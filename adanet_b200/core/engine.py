@@ -1077,6 +1077,7 @@ class IterationPlan:
     self._graph = None
     self._warmed = False      # set by the first (eager) step
     self._stage = None
+    self.carried_overflow = False     # set by a resume from an in-flight state saved after an fp16 overflow
     self.launches_per_step = None
 
   # -- staging -------------------------------------------------------------
@@ -1342,12 +1343,13 @@ class IterationPlan:
         h.load_state_dict({k[len(pre):]: v for k, v in st.items() if k.startswith(pre)})
     torch.cuda.current_stream(self.device).synchronize()
 
-  def plane_overflow(self) -> bool:
-    """True when a finite value did not fit the fp16 planes since the flag was last read (csrc/plane_fmt.cuh); the
-    caller re-runs the iteration on TF32 planes (AdaNetSearch.run / Estimator.train)."""
+  def plane_overflow(self, reset: bool = True) -> bool:
+    """True when a finite value did not fit the fp16 planes since the flag was last read (csrc/plane_fmt.cuh), or the
+    in-flight state this plan resumed from was saved after one (`carried_overflow`); the caller re-runs the iteration
+    on TF32 planes (AdaNetSearch.run / Estimator.train)."""
     if self.fmt != _lib.PLANES_F16 or self.xp is None:
       return False
-    return _lib.plane_overflow(torch.cuda.current_stream(self.device).cuda_stream)
+    return _lib.plane_overflow(torch.cuda.current_stream(self.device).cuda_stream, reset) or self.carried_overflow
 
   # -- read-back ---------------------------------------------------------------
   def _reports(self, h) -> bool:

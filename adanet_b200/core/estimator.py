@@ -368,6 +368,9 @@ class Estimator(object):
     inside the iteration (the reference persists the same through the TF checkpoint,
     adanet/core/iteration.py:40-118,172-183).  Candidate builders are re-generated deterministically on resume."""
     st = self._search.plan.state_dict()
+    st["meta_plane_format"] = np.asarray(self._search.plan.fmt, dtype=np.int64)
+    # the sticky overflow flag, read without clearing it: a run resumed from here must fall back as this one will
+    st["meta_plane_overflow"] = np.asarray(self._search.plan.plane_overflow(reset=False), dtype=np.int64)
     st["meta_iteration"] = np.asarray(self._search.iteration, dtype=np.int64)
     st["meta_global_step"] = np.asarray(self._global_step, dtype=np.int64)
     st["meta_iteration_step"] = np.asarray(self._iteration_step, dtype=np.int64)
@@ -376,14 +379,23 @@ class Estimator(object):
     os.replace(tmp, self._inflight_path())
 
   def _maybe_restore_inflight(self):
-    """Called right after an iteration's plan was built: loads the in-flight state if it belongs to it."""
+    """Called right after an iteration's plan was built: loads the in-flight state if it belongs to it.
+
+    The state belongs to it when it was saved in this iteration, at or after the current global step, on the plan's
+    plane format.  A file on TF32 planes while the plan is on fp16 ones was written by a run that fell back inside this
+    iteration (core/search.py restart_on_tf32_if_overflowed): this process falls back too and rebuilds the plan before
+    loading it.  A file on fp16 planes while the plan is on TF32 ones is a discarded attempt and is refused."""
     if not self._model_dir or self._iteration_step != 0:
       return False
+    from adanet_b200 import _lib
     from adanet_b200.distributed import exchange as ex
+    plan = self._search.plan
     st, ok = None, False
     if os.path.exists(self._inflight_path()):
       st = dict(np.load(self._inflight_path()))
       ok = int(st["meta_iteration"]) == self._search.iteration and int(st["meta_global_step"]) >= self._global_step
+      if ok and plan.xp is not None and self._inflight_format(st) != plan.fmt:
+        ok = self._inflight_format(st) == _lib.PLANES_TF32
     # every rank resumes from the same global step or none does (ranks killed at different save points would otherwise
     # reach the end-of-iteration collectives at different times); all ranks take part in the agreement, file or not
     mine = float(st["meta_global_step"]) if ok else -1.0
@@ -394,7 +406,14 @@ class Estimator(object):
         logging.warning("in-flight checkpoints of the ranks disagree (steps %s..%s): restarting iteration %d", lo, hi,
                         self._search.iteration)
       return False
+    if plan.xp is not None and self._inflight_format(st) != plan.fmt:
+      # every rank saved this step on the same format (the fallback is agreed by all_reduce), so all of them get here
+      logging.warning("iteration %d: the in-flight checkpoint was written on TF32 planes after an fp16 overflow; "
+                      "continuing on TF32 planes", self._search.iteration)
+      _lib.set_plane_format(_lib.PLANES_TF32)
+      self._search.build_iteration()
     self._search.plan.load_state_dict(st)
+    self._search.plan.carried_overflow = bool(int(st.get("meta_plane_overflow", 0)))
     self._global_step = int(st["meta_global_step"])
     self._iteration_step = int(st["meta_iteration_step"])
     for it in getattr(self, "_bagging_iters", {}).values():      # bagging inputs restart with the iteration: skip what it consumed
@@ -403,6 +422,12 @@ class Estimator(object):
     logging.info("resumed iteration %d at iteration step %d (global step %d)", self._search.iteration,
                  self._iteration_step, self._global_step)
     return True
+
+  @staticmethod
+  def _inflight_format(st):
+    """Plane format an in-flight state was saved on; files written before it was recorded were on fp16 planes."""
+    from adanet_b200 import _lib
+    return int(st["meta_plane_format"]) if "meta_plane_format" in st else _lib.PLANES_F16
 
   def _maybe_restore(self):
     """Continues from `model_dir/ensemble-latest.{npz,json}` (written at every iteration boundary): frozen
@@ -428,6 +453,14 @@ class Estimator(object):
                                                                      int(data["global_step"]), int(meta["iteration"]),
                                                                      int(meta["global_step"])))
     s = self._search
+    if meta.get("plane_format") == "tf32":
+      # the run that wrote it fell back from fp16 planes (core/search.py restart_on_tf32_if_overflowed), which is for
+      # good: continue on TF32 as it did.  A checkpoint on fp16 planes, or one written before the format was recorded,
+      # leaves the process's format alone.
+      from adanet_b200 import _lib
+      if _lib.plane_format() != _lib.PLANES_TF32:
+        logging.info("model_dir %s was trained on TF32 planes: switching to them", self._model_dir)
+        _lib.set_plane_format(_lib.PLANES_TF32)
     members = []
     for k, m in enumerate(meta["members"]):
       n_layers = len(m["dims"]) - 1 + (1 if m.get("image_shape") else 0)     # a conv stem's kernel / bias come first
@@ -597,9 +630,12 @@ class Estimator(object):
     s = self._search
     t = s.iteration
     if s.restart_on_tf32_if_overflowed():
-      # the iteration is trained again (TF32 planes) on the input that follows; its steps do not count
+      # the iteration is trained again (TF32 planes) on the input that follows; its steps do not count, and neither
+      # does what the discarded attempt saved in flight (every rank falls back here together and drops its own file)
       self._global_step -= self._iteration_step
       self._iteration_step = 0
+      if self._model_dir and os.path.exists(self._inflight_path()):
+        os.remove(self._inflight_path())
       return None
     builders, subs = self._pending
     if self._evaluator is not None:
@@ -663,8 +699,10 @@ class Estimator(object):
 
   def _save_ensemble(self):
     """The final ensemble's parameters (replaces the reference's increment.ckpt-{t})."""
+    from adanet_b200 import _lib
     s = self._search
-    out = {"global_step": self._global_step, "iteration": s.iteration, "bias": s.bias}
+    fmt = _lib.plane_format()
+    out = {"global_step": self._global_step, "iteration": s.iteration, "bias": s.bias, "plane_format": fmt}
     if isinstance(s.mixture_weights, list):
       for k, w in enumerate(s.mixture_weights):
         out["mixture_weight_{}".format(k)] = w
@@ -688,6 +726,7 @@ class Estimator(object):
         "architecture": [[int(t), n] for t, n in s.architecture], "replay_trace": [int(v) for v in s.replay_trace],
         "prev_best_ema": None if s.prev_best_ema is None else float(s.prev_best_ema),
         "last_candidate_name": self._last_candidate_name, "winner_ens_index": int(s.winner_ens_index),
+        "plane_format": "tf32" if fmt == _lib.PLANES_TF32 else "fp16",
         "members": [{"name": m.name, "iteration": int(m.iteration), "complexity": float(m.complexity),
                      "dims": [int(d) for d in m.dims], "shared": m.shared,
                      "image_shape": list(m.image_shape) if m.stem else None} for m in s.frozen],

@@ -780,9 +780,16 @@ def check_forward(fails, case, c, spec, wsrc, x_in, step_dev, floor, tag, planes
 def check_frozen_forward(fails, fnets, frozen, x, floor, planes=True):
   for k, (f, fs) in enumerate(zip(fnets, frozen)):
     h = f64(x)
+    ws, bs = fs["p"]
+    if f.stem:
+      # a frozen SimpleCNN member: its conv stem from the minibatch, its dense layers from the engine's pooled features
+      st = conv_stem64(np.asarray(x).reshape((f.batch,) + tuple(f.image_shape)), ws[0], bs[0])
+      h = _merge(f.stem_out, f.batch, f.dims[0])
+      _check(fails, "forward", h, st["pooled"], st["bound"] + floor, "frozen %d conv stem" % k)
+      ws, bs = ws[1:], bs[1:]
     acts = _acts(f, f.batch, planes)
-    for i, (w, b) in enumerate(zip(*fs["p"])):
-      last = i == len(fs["p"][0]) - 1
+    for i, (w, b) in enumerate(zip(ws, bs)):
+      last = i == len(ws) - 1
       exact, bound = layer_fwd(h, w, b, not last, floor=floor, fp32_dot=not planes)
       got = f.logits.cpu().numpy() if last else acts[i]
       _check(fails, "forward", got, exact, bound, "frozen %d layer %d" % (k, i))
@@ -1018,10 +1025,11 @@ def _members(case, plan, fnets, gidx, h):
   """the nets candidate ensemble `gidx` must read, from the case description (not from the head itself): the kept
   frozen members, then the new subnetworks it names (GrowStrategy: every frozen member and its own candidate)"""
   from adanet_b200.core import engine as eng
+  by_index = {c.index: c.net for c in plan.candidates}      # a rank of a multi-rank search holds some candidates only
   if case.get("heads"):
     _, builders, keep, _ = case["heads"][gidx]
-    return [fnets[i] for i in eng.kept_indices(keep, len(fnets))] + [plan.candidates[b].net for b in builders]
-  return list(fnets) + [plan.candidates[gidx].net]
+    return [fnets[i] for i in eng.kept_indices(keep, len(fnets))] + [by_index[b] for b in builders]
+  return list(fnets) + [by_index[gidx]]
 
 
 def check_head(fails, case, plan, fnets, gidx, h, pre, post, x, y, step_dev, cap, tag, planes, f16):
