@@ -36,12 +36,21 @@ EXPORTS = (
 )
 
 
+FWD_MAX_SRCS = 3      # ADN_FWD_MAX_SRCS
+
+
+class FwdSrc(ctypes.Structure):
+  """adn_fwd_src (include/adanet_b200.h): one more input piece of a multi-source forward op"""
+  _fields_ = [("xp", c_void_p), ("wp", c_void_p), ("in_", c_int64)]
+
+
 class FwdOp(ctypes.Structure):
   """adn_fwd_op (include/adanet_b200.h)"""
   _fields_ = [("xp", c_void_p), ("wp", c_void_p), ("bias", c_void_p), ("yp", c_void_p), ("y", c_void_p),
               ("in_", c_int64), ("out", c_int64), ("act", ctypes.c_int32), ("reserved", ctypes.c_int32),
               ("dropout_rate", c_float), ("dropout_seed", ctypes.c_uint32), ("dropout_layer", ctypes.c_int32),
-              ("dropout_row0", ctypes.c_int32), ("dropout_step_dev", c_void_p)]
+              ("dropout_row0", ctypes.c_int32), ("dropout_step_dev", c_void_p),
+              ("srcs", POINTER(FwdSrc)), ("n_srcs", ctypes.c_int32), ("reserved3", ctypes.c_int32)]
 
 
 class BwdOp(ctypes.Structure):

@@ -226,14 +226,34 @@ extern "C" int adn_dense_fwd_p_group(const adn_fwd_op* ops, int n, int64_t batch
   if (n < 0 || (n > 0 && !ops)) return fail(ADN_ERR_INVALID, "adn_dense_fwd_p_group: bad ops");
   if (n > 256) return fail(ADN_ERR_UNSUPPORTED, "adn_dense_fwd_p_group: n %d > 256", n);
   pl::FwdOp o[256];
+  pl::FwdSrc srcs[256][ADN_FWD_MAX_SRCS];
   for (int i = 0; i < n; ++i) {
     if (!ops[i].xp || !ops[i].wp) return fail(ADN_ERR_INVALID, "adn_dense_fwd_p_group: op %d: null pointer", i);
+    const int ns = ops[i].n_srcs;
+    if (ns < 0 || ns > ADN_FWD_MAX_SRCS || (ns > 0 && !ops[i].srcs))
+      return fail(ADN_ERR_INVALID, "adn_dense_fwd_p_group: op %d: n_srcs %d (0..%d, srcs non-NULL)", i, ns, ADN_FWD_MAX_SRCS);
+    int64_t k_total = ops[i].in;
+    for (int q = 0; q < ns; ++q) {
+      const adn_fwd_src& s = ops[i].srcs[q];
+      if (!s.xp || !s.wp) return fail(ADN_ERR_INVALID, "adn_dense_fwd_p_group: op %d: piece %d: null pointer", i, q);
+      if (bad_shape(batch, s.in, ops[i].out))
+        return fail(ADN_ERR_INVALID, "adn_dense_fwd_p_group: op %d: piece %d: bad shape (in %lld)", i, q, (long long)s.in);
+      if (!pl::planes_aligned(s.xp) || !pl::planes_aligned(s.wp))
+        return fail(ADN_ERR_INVALID, "adn_dense_fwd_p_group: op %d: piece %d: plane buffers must be 256 B aligned", i, q);
+      srcs[i][q] = pl::FwdSrc{s.xp, s.wp, s.in};
+      k_total += s.in;
+    }
+    if (ns > 0 && k_total > INT32_MAX) return fail(ADN_ERR_INVALID, "adn_dense_fwd_p_group: op %d: total K too large", i);
     if ((ops[i].yp == nullptr) == (ops[i].y == nullptr))
       return fail(ADN_ERR_INVALID, "adn_dense_fwd_p_group: op %d: exactly one of yp / y", i);
     if (bad_shape(batch, ops[i].in, ops[i].out)) return fail(ADN_ERR_INVALID, "adn_dense_fwd_p_group: op %d: bad shape", i);
     if (ops[i].act != ADN_ACT_NONE && ops[i].act != ADN_ACT_RELU)
       return fail(ADN_ERR_INVALID, "adn_dense_fwd_p_group: op %d: bad act %d", i, ops[i].act);
     o[i] = pl::FwdOp{ops[i].xp, ops[i].wp, ops[i].bias, ops[i].yp, ops[i].y, ops[i].in, ops[i].out, ops[i].act};
+    if (ns > 0) {
+      o[i].srcs = srcs[i];
+      o[i].n_srcs = ns;
+    }
     if (ops[i].dropout_rate != 0.f) {
       if (!(ops[i].dropout_rate > 0.f && ops[i].dropout_rate < 1.f) || !ops[i].yp || !ops[i].dropout_step_dev)
         return fail(ADN_ERR_INVALID, "adn_dense_fwd_p_group: op %d: dropout needs 0 < rate < 1, planes out and a step counter", i);

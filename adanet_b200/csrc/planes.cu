@@ -47,6 +47,7 @@
 #include <atomic>
 #include <mutex>
 #include <string>
+#include <type_traits>
 #include <unordered_map>
 #include <vector>
 
@@ -577,16 +578,39 @@ struct alignas(64) Group {
   int total_items;
 };
 
+// Multi-source forward: y = act(x_0 w_0 + sum_s x_s w_s + b), the dense layer over a concatenation of its inputs.
+// Every piece is its own plane tensor zero-padded in its own K tail, so the K loop runs over sum_p ceil(in_p / BK)
+// k-blocks and the producer switches descriptors at piece boundaries; the consumers and the epilogue do not see the
+// pieces.  A separate parameter block and instantiation leave the single-source parameter block (Group) as it is.
+static constexpr int MAX_SRCS = ADN_FWD_MAX_SRCS;     // pieces besides (xp, wp)
+struct alignas(64) MsProblem {
+  CUtensorMap a_hi, a_lo, b_hi, b_lo;       // piece 0: the op's own xp / wp
+  CUtensorMap o_hi, o_lo;
+  CUtensorMap src[MAX_SRCS][4];             // pieces 1..n_src: a_hi, a_lo, b_hi, b_lo
+  GemmParams g;
+  int item0;
+  int n_src;
+  int kb_end[MAX_SRCS + 1];                 // k-block at which piece p ends (cumulative); kb_end[n_src] = g.total_kb
+};
+struct alignas(64) MsGroup {
+  MsProblem p[MAX_GROUP];
+  int n;
+  int total_items;
+};
+static_assert(sizeof(MsGroup) <= 32764, "kernel parameter space");
+
 // advance `cur` to the problem that owns `item` (items are visited in increasing order).  `next0` caches the first item
 // of the following problem in a register: the common case is one compare, not an indexed load from the parameter bank.
-__device__ __forceinline__ int find_problem(const Group& grp, int cur, int item, int& next0) {
+template <class G>
+__device__ __forceinline__ int find_problem(const G& grp, int cur, int item, int& next0) {
   while (item >= next0) {
     ++cur;
     next0 = (cur + 1 < grp.n) ? grp.p[cur + 1].item0 : 0x7fffffff;
   }
   return cur;
 }
-__device__ __forceinline__ int first_next0(const Group& grp) { return grp.n > 1 ? grp.p[1].item0 : 0x7fffffff; }
+template <class G>
+__device__ __forceinline__ int first_next0(const G& grp) { return grp.n > 1 ? grp.p[1].item0 : 0x7fffffff; }
 
 // One work item as the epilogue warpgroup sees it, with the global values its slices need: the ReLU-mask words of
 // the lane's row for the two 32-column halves (EPI_MASK; all ones without a mask, 0 past M or the last 32-column
@@ -597,8 +621,8 @@ struct EpiItem {
   uint32_t mw0, mw1;
   uint32_t drop_step;
 };
-template <int EPI>
-__device__ __forceinline__ EpiItem epi_fetch(const Group& grp, int& cur, int& next0, int item, int tile_row) {
+template <int EPI, class G>
+__device__ __forceinline__ EpiItem epi_fetch(const G& grp, int& cur, int& next0, int item, int tile_row) {
   EpiItem e;
   cur = find_problem(grp, cur, item, next0);
   e.p = cur;
@@ -701,9 +725,10 @@ __device__ __forceinline__ void tf32_kblock(const uint8_t* st, int arow0, int la
     }
   }
 }
-template <int FMT, int EPI>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
-pl_gemm_kernel(const __grid_constant__ Group grp) {
+// The kernel body, shared by pl_gemm_kernel (Group) and pl_gemm_ms_kernel (MsGroup, forward only).
+template <int FMT, int EPI, class G>
+__device__ __forceinline__ void pl_gemm_body(const G& grp) {
+  constexpr bool MS = std::is_same<G, MsGroup>::value;
   constexpr int BK = Fmt<FMT>::BK;
   constexpr int CHUNK = Fmt<FMT>::CHUNK;
   constexpr int A_MN = EPI == EPI_PARTIAL, B_MN = EPI != EPI_MASK;   // operand majorness of fwd / dX / dW
@@ -738,6 +763,10 @@ pl_gemm_kernel(const __grid_constant__ Group grp) {
     tma_prefetch_desc(&grp.p[lane].a_lo);
     tma_prefetch_desc(&grp.p[lane].b_hi);
     tma_prefetch_desc(&grp.p[lane].b_lo);
+    if constexpr (MS) {
+      for (int q = 0; q < grp.p[lane].n_src; ++q)
+        for (int m = 0; m < 4; ++m) tma_prefetch_desc(&grp.p[lane].src[q][m]);
+    }
   }
   __syncthreads();
 
@@ -750,22 +779,40 @@ pl_gemm_kernel(const __grid_constant__ Group grp) {
       const uint32_t smem0 = smem_u32(smem);
       for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
         cur = find_problem(grp, cur, item, next0);
-        const Problem& pr = grp.p[cur];
+        const auto& pr = grp.p[cur];
         const GemmParams& g = pr.g;
         const Item it = decode_item(g, item - pr.item0);
+        // multi-source: the piece q of k-block kc, its first k-block and its end.  Multi-source problems have one
+        // split (kb0 = 0), k-blocks are visited in order and every piece has at least one, so q advances by at most
+        // one per k-block and the parameter block is read only at piece boundaries.
+        [[maybe_unused]] int q = 0, q_kb0 = 0, q_end = 0;
+        if constexpr (MS) q_end = pr.kb_end[0];
         for (int kb = 0; kb < it.nkb; ++kb) {
           mbar_wait(smem_u32(&empty_bar[s]), ph ^ 1);
           const uint32_t fb = smem_u32(&full_bar[s]);
           mbar_expect_tx(fb, STAGE_BYTES);
           const uint32_t base = smem0 + s * STAGE_BYTES;
-          const int kc = it.kb0 + kb;
+          int kc = it.kb0 + kb;
+          const CUtensorMap *a_hi = &pr.a_hi, *a_lo = &pr.a_lo, *b_hi = &pr.b_hi, *b_lo = &pr.b_lo;
+          if constexpr (MS) {       // kc inside its piece
+            if (kc >= q_end) {
+              ++q;
+              q_kb0 = q_end;
+              q_end = pr.kb_end[q];
+            }
+            if (q > 0) {
+              kc -= q_kb0;
+              a_hi = &pr.src[q - 1][0]; a_lo = &pr.src[q - 1][1];
+              b_hi = &pr.src[q - 1][2]; b_lo = &pr.src[q - 1][3];
+            }
+          }
           // K-major box {BK, rows, 1 kb} at (0, row0, kc); MN-major box {BK, BK rows, rows/BK kb} at (0, kc*BK, mn0/BK)
           const int a1 = A_MN ? kc * BK : it.m0, a2 = A_MN ? (it.m0 / BK) : kc;
           const int b1 = B_MN ? kc * BK : it.n0, b2 = B_MN ? (it.n0 / BK) : kc;
-          tma_load_3d(&pr.a_hi, fb, base, 0, a1, a2);
-          tma_load_3d(&pr.a_lo, fb, base + A_TILE, 0, a1, a2);
-          tma_load_3d(&pr.b_hi, fb, base + 2 * A_TILE, 0, b1, b2);
-          tma_load_3d(&pr.b_lo, fb, base + 2 * A_TILE + B_TILE, 0, b1, b2);
+          tma_load_3d(a_hi, fb, base, 0, a1, a2);
+          tma_load_3d(a_lo, fb, base + A_TILE, 0, a1, a2);
+          tma_load_3d(b_hi, fb, base + 2 * A_TILE, 0, b1, b2);
+          tma_load_3d(b_lo, fb, base + 2 * A_TILE + B_TILE, 0, b1, b2);
           if (++s == STAGES) { s = 0; ph ^= 1; }
         }
       }
@@ -888,6 +935,17 @@ pl_gemm_kernel(const __grid_constant__ Group grp) {
     }
     mbar_arrive(smem_u32(&tile_full[buf]));
   }
+}
+
+template <int FMT, int EPI>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+pl_gemm_kernel(const __grid_constant__ Group grp) {
+  pl_gemm_body<FMT, EPI>(grp);
+}
+template <int FMT>
+__global__ void __launch_bounds__(NUM_THREADS, 1)
+pl_gemm_ms_kernel(const __grid_constant__ MsGroup grp) {
+  pl_gemm_body<FMT, EPI_BIAS_ACT>(grp);
 }
 
 // ---------------------------------------------------------------------------------
@@ -1026,6 +1084,8 @@ int init() {
     ADN_PL_ATTR(FMT_TF32, EPI_BIAS_ACT); ADN_PL_ATTR(FMT_TF32, EPI_MASK); ADN_PL_ATTR(FMT_TF32, EPI_PARTIAL);
     ADN_PL_ATTR(FMT_F16, EPI_BIAS_ACT); ADN_PL_ATTR(FMT_F16, EPI_MASK); ADN_PL_ATTR(FMT_F16, EPI_PARTIAL);
 #undef ADN_PL_ATTR
+    ok = ok && cudaFuncSetAttribute(pl_gemm_ms_kernel<FMT_TF32>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) == cudaSuccess;
+    ok = ok && cudaFuncSetAttribute(pl_gemm_ms_kernel<FMT_F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) == cudaSuccess;
     if (!ok) {
       (void)cudaGetLastError();
       rc = fail(ADN_ERR_CUDA, "pl::init: cudaFuncSetAttribute(smem=%d) failed", SMEM_BYTES);
@@ -1151,12 +1211,13 @@ static int store_mode() {      // ADN_PL_TMA_STORE=0: direct global stores inste
 struct GemmDesc {
   Operand a, b;
   GemmParams g;
+  int n_src = 0;                       // multi-source forward: pieces (x, w) besides (a, b)
+  Operand sa[MAX_SRCS], sb[MAX_SRCS];
 };
 
 static int encode_maps(int fmt, const GemmDesc& d, CUtensorMap* a_hi, CUtensorMap* a_lo, CUtensorMap* b_hi, CUtensorMap* b_lo,
                        const char* what) {
-  if ((reinterpret_cast<uintptr_t>(d.a.hi) | reinterpret_cast<uintptr_t>(d.a.lo) | reinterpret_cast<uintptr_t>(d.b.hi) |
-       reinterpret_cast<uintptr_t>(d.b.lo)) & 127)
+  if (!planes_aligned(d.a.hi) || !planes_aligned(d.a.lo) || !planes_aligned(d.b.hi) || !planes_aligned(d.b.lo))
     return fail(ADN_ERR_INVALID, "%s: plane buffers must be 256 B aligned", what);
   int rc;
   if ((rc = make_map(fmt, a_hi, d.a.hi, d.a.rows, d.a.nkb, d.a.mn_major, BM))) return rc;
@@ -1180,23 +1241,43 @@ template <int FMT, int EPI>
 static void launch_kernel(const Group& grp, int grid, cudaStream_t st) {
   pl_gemm_kernel<FMT, EPI><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(grp);
 }
-// n independent GEMMs of the same epilogue kind -> persistent launches of up to MAX_GROUP problems each
-template <int EPI>
-static int launch_group(int fmt, const GemmDesc* d, int n, cudaStream_t st, const char* what) {
+// n independent GEMMs of the same epilogue kind -> parameter blocks of up to MAX_GROUP problems each, one per
+// persistent launch (G = MsGroup: multi-source forward GEMMs, on pl_gemm_ms_kernel).  Every descriptor is encoded
+// here, before anything is launched, so that a failure leaves every output as it was.
+template <int EPI, class G>
+static int build_groups(int fmt, const GemmDesc* d, int n, std::vector<G>& out, const char* what) {
+  constexpr bool MS = std::is_same<G, MsGroup>::value;
+  static_assert(!MS || EPI == EPI_BIAS_ACT, "multi-source GEMMs are forward only");
+  out.clear();
   {
     for (int i0 = 0; i0 < n; i0 += MAX_GROUP) {
       const int m = std::min(MAX_GROUP, n - i0);
-      Group grp;
+      out.emplace_back();
+      G& grp = out.back();
       memset(&grp, 0, sizeof(grp));
       int items = 0;
       for (int i = 0; i < m; ++i) {
         const GemmDesc& src = d[i0 + i];
-        Problem& pr = grp.p[i];
+        auto& pr = grp.p[i];
         // the kernel fixes the operand majorness per epilogue kind (fwd: K / MN, dX: K / K, dW: MN / MN)
         if (src.a.mn_major != (EPI == EPI_PARTIAL) || src.b.mn_major != (EPI != EPI_MASK))
           return fail(ADN_ERR_INVALID, "%s: operand majorness does not match the epilogue kind", what);
         int rc = encode_maps(fmt, src, &pr.a_hi, &pr.a_lo, &pr.b_hi, &pr.b_lo, what);
         if (rc) return rc;
+        if constexpr (MS) {
+          int kb = (int)src.a.nkb;
+          pr.n_src = src.n_src;
+          pr.kb_end[0] = kb;
+          for (int q = 0; q < src.n_src; ++q) {
+            GemmDesc piece;
+            piece.a = src.sa[q];
+            piece.b = src.sb[q];
+            if ((rc = encode_maps(fmt, piece, &pr.src[q][0], &pr.src[q][1], &pr.src[q][2], &pr.src[q][3], what))) return rc;
+            kb += (int)src.sa[q].nkb;
+            pr.kb_end[q + 1] = kb;
+          }
+          if (kb != src.g.total_kb) return fail(ADN_ERR_INVALID, "%s: k-blocks of the pieces do not add up", what);
+        }
         pr.g = src.g;
         pr.g.out_tma = 0;
         if (fmt == FMT_F16 && EPI != EPI_PARTIAL && src.g.out_planes && store_mode() && (src.g.out_nb32 & 1) == 0 &&
@@ -1222,13 +1303,30 @@ static int launch_group(int fmt, const GemmDesc* d, int n, cudaStream_t st, cons
       }
       grp.n = m;
       grp.total_items = items;
-      const int grid = std::min(items, sm_count());
-      if (fmt == FMT_F16) launch_kernel<FMT_F16, EPI>(grp, grid, st);
-      else launch_kernel<FMT_TF32, EPI>(grp, grid, st);
-      ADN_CHECK_LAUNCH(what);
     }
   }
   return ADN_OK;
+}
+template <int EPI, class G>
+static int launch_groups(int fmt, const std::vector<G>& groups, cudaStream_t st, const char* what) {
+  for (const G& grp : groups) {
+    const int grid = std::min(grp.total_items, sm_count());
+    if constexpr (std::is_same<G, MsGroup>::value) {
+      if (fmt == FMT_F16) pl_gemm_ms_kernel<FMT_F16><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(grp);
+      else pl_gemm_ms_kernel<FMT_TF32><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(grp);
+    } else {
+      if (fmt == FMT_F16) launch_kernel<FMT_F16, EPI>(grp, grid, st);
+      else launch_kernel<FMT_TF32, EPI>(grp, grid, st);
+    }
+    ADN_CHECK_LAUNCH(what);
+  }
+  return ADN_OK;
+}
+template <int EPI>
+static int launch_group(int fmt, const GemmDesc* d, int n, cudaStream_t st, const char* what) {
+  std::vector<Group> groups;
+  const int rc = build_groups<EPI>(fmt, d, n, groups, what);
+  return rc ? rc : launch_groups<EPI>(fmt, groups, st, what);
 }
 
 int split(int fmt, const float* src, int64_t rows, int64_t cols, void* planes, int log2_scale, cudaStream_t st) {
@@ -1276,15 +1374,23 @@ int64_t dense_bwd_workspace_bytes(int64_t batch, int64_t in, int64_t out) {
 int dense_fwd_group(int fmt, const FwdOp* ops, int n, int64_t batch, cudaStream_t st) {
   if (n <= 0) return ADN_OK;
   const int bk = fmt_bk(fmt);
-  std::vector<GemmDesc> d((size_t)n);
+  std::vector<GemmDesc> d, dm;     // single-source ops, multi-source ops
+  d.reserve((size_t)n);
   for (int i = 0; i < n; ++i) {
     const FwdOp& o = ops[i];
-    GemmDesc& e = d[(size_t)i];
+    GemmDesc e;
     e.a = operand(fmt, o.xp, batch, o.in, 0);       // A = x  [M=batch, K=in]  K-major
     e.b = operand(fmt, o.wp, o.in, o.out, 1);       // B = w  [K=in, N=out]    MN-major
+    int64_t kb = ceil_div(o.in, bk);
+    e.n_src = o.n_srcs;
+    for (int q = 0; q < o.n_srcs; ++q) {             // piece q: x_q [batch, in_q] times rows of w [in_q, out]
+      e.sa[q] = operand(fmt, o.srcs[q].xp, batch, o.srcs[q].in, 0);
+      e.sb[q] = operand(fmt, o.srcs[q].wp, o.srcs[q].in, o.out, 1);
+      kb += ceil_div(o.srcs[q].in, bk);
+    }
     GemmParams g{};
     g.M = (int)batch; g.N = (int)o.out;
-    g.total_kb = (int)ceil_div(o.in, bk); g.kb_per_split = g.total_kb; g.splits = 1;
+    g.total_kb = (int)kb; g.kb_per_split = g.total_kb; g.splits = 1;
     g.bias = o.bias; g.act = o.act;
     g.out_mul = 1.0f;
     if (o.dropout_rate > 0.f) {
@@ -1306,8 +1412,16 @@ int dense_fwd_group(int fmt, const FwdOp* ops, int n, int64_t batch, cudaStream_
       g.out = o.y; g.ldc = (int)o.out;
     }
     e.g = g;
+    (o.n_srcs ? dm : d).push_back(e);
   }
-  return launch_group<EPI_BIAS_ACT>(fmt, d.data(), n, st, "pl dense_fwd gemm");
+  // both kinds are encoded before either is launched: a call that returns an error has written nothing
+  std::vector<Group> groups;
+  std::vector<MsGroup> ms_groups;
+  int rc;
+  if ((rc = build_groups<EPI_BIAS_ACT>(fmt, d.data(), (int)d.size(), groups, "pl dense_fwd gemm"))) return rc;
+  if ((rc = build_groups<EPI_BIAS_ACT>(fmt, dm.data(), (int)dm.size(), ms_groups, "pl dense_fwd multi-source gemm"))) return rc;
+  if ((rc = launch_groups<EPI_BIAS_ACT>(fmt, groups, st, "pl dense_fwd gemm"))) return rc;
+  return launch_groups<EPI_BIAS_ACT>(fmt, ms_groups, st, "pl dense_fwd multi-source gemm");
 }
 
 int dense_bwd_group(int fmt, const BwdOp* ops, int n, int64_t batch, cudaStream_t st) {

@@ -17,6 +17,11 @@ int64_t dense_bwd_workspace_bytes(int64_t batch, int64_t in, int64_t out);
 int split(int fmt, const float* src, int64_t rows, int64_t cols, void* planes, int log2_scale, cudaStream_t st);
 int merge(int fmt, const void* planes, int64_t rows, int64_t cols, float* dst, cudaStream_t st);
 // one dense layer of one subnetwork; groups = the same layer wave of several subnetworks in one launch
+struct FwdSrc {         // one more input piece of a multi-source forward (include/adanet_b200.h adn_fwd_src)
+  const void* xp;       // planes [batch, in]
+  const void* wp;       // planes [in, out]
+  int64_t in;
+};
 struct FwdOp {
   const void* xp;       // planes [batch, in]
   const void* wp;       // planes [in, out]
@@ -30,6 +35,8 @@ struct FwdOp {
   int dropout_layer = 0;
   int64_t dropout_row0 = 0;          // first minibatch row of a row slice: the mask is the full batch's
   const int64_t* dropout_step = nullptr;
+  const FwdSrc* srcs = nullptr;      // y = act(x w + sum_q srcs[q].x srcs[q].w + b), n_srcs <= ADN_FWD_MAX_SRCS
+  int n_srcs = 0;
 };
 struct BwdOp {
   const void* xp;       // planes [batch, in]
@@ -46,6 +53,9 @@ struct BwdOp {
   int64_t ws_bytes;
   float dx_mul = 1.f;   // dx (planes or dense) is multiplied by this: 1 / (1 - rate) below a dropped-out activation
 };
+// The alignment every GEMM operand plane is checked against (include/adanet_b200.h asks callers for 256 B; the TMA
+// descriptors need 128 B).
+inline bool planes_aligned(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 127) == 0; }
 int dense_fwd_group(int fmt, const FwdOp* ops, int n, int64_t batch, cudaStream_t st);
 int dense_bwd_group(int fmt, const BwdOp* ops, int n, int64_t batch, cudaStream_t st);
 // exactly one of yp (planes out) / y (dense fp32 out) is non-null

@@ -226,6 +226,16 @@ int adn_dense_bwd_p(const void* xp, const void* wp, const void* dzp, void* dxp, 
  * prologue and pipeline fill/drain are paid once per wave and narrow candidates hide behind wide ones.
  * Per-op semantics are exactly adn_dense_fwd_p / adn_dense_bwd_p; ops must not alias each other's outputs.
  */
+/* One more input piece of a multi-source forward op: planes xp [batch, in] and the matching rows of the layer's
+ * kernel as their own planes wp [in, out].  A dense layer over concat([x_0, x_1, ...], axis=-1) with kernel
+ * W = [W_0; W_1; ...] (row blocks in the same order) is y = act(x_0 W_0 + x_1 W_1 + ... + b): AdaNet subnetworks
+ * that read the hidden layers of earlier subnetworks (Cortes et al., ICML 2017; adanet/subnetwork/generator.py:96-105). */
+typedef struct adn_fwd_src {
+  const void* xp;
+  const void* wp;
+  int64_t in;          /* > 0 */
+} adn_fwd_src;
+#define ADN_FWD_MAX_SRCS 3 /* pieces per op besides (xp, wp) */
 typedef struct adn_fwd_op {
   const void* xp;      /* planes [batch, in]  */
   const void* wp;      /* planes [in, out]    */
@@ -246,6 +256,14 @@ typedef struct adn_fwd_op {
   int32_t dropout_layer;
   int32_t dropout_row0;
   const int64_t* dropout_step_dev;
+  /* Multi-source forward: y = act(xp wp + sum_{s < n_srcs} srcs[s].xp srcs[s].wp + b), K = in + sum_s srcs[s].in.
+   * 0 <= n_srcs <= ADN_FWD_MAX_SRCS (srcs may be NULL when 0).  Ops with n_srcs > 0 run on a launch of their own,
+   * so a group that mixes both kinds takes one launch per kind (per 8 ops); the epilogue (bias, ReLU, sign bits,
+   * dropout, planes or dense out) is the same.  A negative or too large n_srcs, a NULL piece pointer, in <= 0 or
+   * a misaligned plane buffer is ADN_ERR_INVALID before any op of the call is launched. */
+  const adn_fwd_src* srcs;
+  int32_t n_srcs;
+  int32_t reserved3;
 } adn_fwd_op;
 typedef struct adn_bwd_op {
   const void* xp;      /* planes [batch, in]  */
