@@ -7,27 +7,28 @@ candidate ensemble's train op in one `session.run` per step through hooks
 (adanet/core/iteration.py:150-205,961-996).  Here an :class:`IterationPlan`
 owns, for the candidates placed on this GPU, all parameters, activations,
 gradients and bookkeeping in HBM and enqueues the hand-written sm_90a (H100) kernels
-of ``adanet_b200/csrc`` through the C ABI (include/adanet_b200.h):
-
-  frozen members  -> adn_dense_fwd (forward-only replay, shared by all candidates)
-  new subnetwork  -> adn_dense_fwd / adn_head_loss / adn_dense_bwd / adn_opt_step
-  candidate head  -> adn_ensemble_head (+ adn_opt_step on the mixture weights)
-  EMA / steps     -> adn_ema_update / adn_record_scalars / adn_counter_add
+of ``adanet_b200/csrc`` through the C ABI (include/adanet_b200.h).
 
 Dense layers run on the plane-native tensor-core pipeline (csrc/planes.cu): the
 minibatch is split into hi/lo planes (fp16 pairs by default, TF32 pairs as the
-fallback: csrc/plane_fmt.cuh) once per step, every hidden activation and
-back-propagated gradient stays in plane format between GEMMs
-(adn_dense_fwd_p_group / adn_dense_bwd_p_group), the subnetwork losses and the
-candidate-ensemble heads of all candidates run in one grouped launch
-(adn_head_group), and one grouped optimizer launch updates every parameter and
-refreshes the weight planes (adn_opt_step_group).  With ADN_DENSE_PATH=simt the fp32 CUDA-core ABI
-(adn_dense_fwd / adn_dense_bwd) is used instead, as an on-device cross-check.
+fallback: csrc/plane_fmt.cuh) once per step and every hidden activation and
+back-propagated gradient stays in plane format between GEMMs.  A step is a wave
+schedule (IterationPlan._enqueue_waves) of grouped launches built from one op
+builder per stage:
+
+  forward layer   -> DenseNet.fwd_op          in adn_dense_fwd_p_group (frozen members too)
+  losses, heads   -> CandidatePlan.sub_head_op / EnsembleHead.head_op in adn_head_group
+  backward layer  -> CandidatePlan.bwd_op     in adn_dense_bwd_p_group
+  optimizers      -> _Optimizer.op            in adn_opt_step_group
+  EMA / trace     -> EnsembleHead.book        in adn_head_bookkeeping
+
+With ADN_DENSE_PATH=simt the fp32 CUDA-core ABI is used instead, as an on-device
+cross-check: each candidate runs its whole step op by op (adn_dense_fwd /
+adn_head_loss / adn_ensemble_head / adn_dense_bwd / adn_opt_step) on its own
+stream (CandidatePlan.enqueue_simt_step).
 
 Once shapes are fixed the whole step is captured in a CUDA graph, so a step is
-one graph launch (the fp32 SIMT cross-check path still runs each candidate on
-its own stream).  PyTorch is used for device memory,
-streams and graphs only.
+one graph launch.  PyTorch is used for device memory, streams and graphs only.
 """
 
 from __future__ import annotations
@@ -125,6 +126,25 @@ def kept_indices(keep_previous, n_frozen: int) -> List[int]:
   if any(i < 0 or i >= n_frozen for i in idx) or sorted(set(idx)) != idx:
     raise ValueError("kept previous members must be increasing indices below %d, got %r" % (n_frozen, idx))
   return idx
+
+
+def gammas(lam: float, beta: float, complexities: Sequence[float]) -> List[float]:
+  """gamma_k = lambda * complexity_k + beta of each member (weighted.py:351-358, _compute_adanet_gamma), evaluated in
+  fp32 like the graph does."""
+  return [float(np.float32(beta) if lam == 0.0 else np.float32(np.float32(lam) * np.float32(c) + np.float32(beta)))
+          for c in complexities]
+
+
+def matrix_member_logits(lib, members, mwp, mw_logits, xp, sp: int, mw=None, mw_l1=None):
+  """MATRIX mixture weights (weighted.py:449): weighted_k = last_layer_k @ W_k of every member by the plane GEMM, into
+  mw_logits[k]; with `mw`, also ||W_k||_1 into mw_l1[k] for the regulariser, right after member k's GEMM."""
+  for k, m in enumerate(members):
+    batch, C = mw_logits[k].shape
+    _lib.check(lib.adn_dense_fwd_p(m.last_layer_planes(xp).data_ptr(), mwp[k].data_ptr(), None, None,
+                                   mw_logits[k].data_ptr(), batch, m.last_layer_dim, C, _lib.ACT_NONE, sp),
+               "adn_dense_fwd_p")
+    if mw is not None:
+      _lib.check(lib.adn_l1_norm(mw[k].data_ptr(), mw[k].numel(), mw_l1.data_ptr() + 4 * k, sp), "adn_l1_norm")
 
 
 def _select_prev(prev_mixture_weights, idx: List[int]):
@@ -308,14 +328,8 @@ class _Optimizer:
                       cast(self._cols, ctypes.c_int64) if self.planes is not None else None)
 
   def apply(self, lib, grads: List[torch.Tensor], stream_ptr: int):
-    g = _lib.ptr_array([t.data_ptr() for t in grads])
-    step = self.step_dev.data_ptr() if self.step_dev is not None else None
-    if self.planes is not None:
-      _lib.check(lib.adn_opt_step_p(self.kind, self._p, g, self._s0, self._s1, self._sizes, len(self.params),
-                                    self._hyper, step, self._planes, self._cols, stream_ptr), "adn_opt_step_p")
-    else:
-      _lib.check(lib.adn_opt_step(self.kind, self._p, g, self._s0, self._s1, self._sizes, len(self.params),
-                                  self._hyper, step, stream_ptr), "adn_opt_step")
+    """This update alone: a one-op adn_opt_step_group."""
+    _lib.check(lib.adn_opt_step_group((_lib.OptOp * 1)(self.op(grads)), 1, stream_ptr), "adn_opt_step_group")
 
 
 class DenseNet:
@@ -463,18 +477,11 @@ class DenseNet:
     """x: dense fp32 minibatch; xp: its split planes (required on the plane path)."""
     n = len(self.ws)
     if self.planes:
-      hp = xp
       if self.stem:
         self.stem_forward(lib, x, sp)
-        hp = self.stem_out
       for i in range(n):
-        last = i == n - 1
-        _lib.check(lib.adn_dense_fwd_p(hp.data_ptr(), self.wps[i].data_ptr(), self.bs[i].data_ptr(),
-                                       None if last else self.hp[i].data_ptr(),
-                                       self.acts[i].data_ptr() if last else None, self.batch, self.dims[i],
-                                       self.dims[i + 1], _lib.ACT_NONE if last else _lib.ACT_RELU, sp),
-                   "adn_dense_fwd_p")
-        hp = None if last else self.hp[i]
+        _lib.check(lib.adn_dense_fwd_p_group((_lib.FwdOp * 1)(self.fwd_op(i, xp)), 1, self.batch, sp),
+                   "adn_dense_fwd_p_group")
       return
     h = x
     for i in range(n):
@@ -578,9 +585,7 @@ class EnsembleHead:
     if self.kind == "mean":
       lam = beta = 0.0
     self.reg_is_zero = int(lam == 0.0 and beta == 0.0)
-    # weighted.py:351-358 (_compute_adanet_gamma), evaluated in fp32 like the graph does
-    self.gammas = [float(np.float32(beta) if lam == 0.0 else np.float32(np.float32(lam) * np.float32(c) + np.float32(beta)))
-                   for c in self.complexities]
+    self.gammas = gammas(lam, beta, self.complexities)
     self.reg_multiplier = 1.0 if ens.legacy_train_op else 2.0   # SURVEY.md section 3.3 step 11
     self.out3 = alloc((3,))
     self.ens_opt = None
@@ -615,16 +620,6 @@ class EnsembleHead:
     self._trace_src = _lib.ptr_array([src0.data_ptr(), self.out3.data_ptr(), self.out3.data_ptr() + 8,
                                       self.ema_state.data_ptr() + 8])
 
-  def matrix_forward(self, xp, sp: int):
-    """weighted.py:449: weighted_k = last_layer_k @ W_k for every member, and ||W_k||_1 for the regulariser."""
-    lib, B, C = self.lib, self.batch, self.C
-    for k, m in enumerate(self.member_nets):
-      _lib.check(lib.adn_dense_fwd_p(m.last_layer_planes(xp).data_ptr(), self.mwp[k].data_ptr(), None, None,
-                                     self.mw_logits[k].data_ptr(), B, m.last_layer_dim, C, _lib.ACT_NONE, sp),
-                 "adn_dense_fwd_p")
-      _lib.check(lib.adn_l1_norm(self.mw[k].data_ptr(), self.mw[k].numel(), self.mw_l1.data_ptr() + 4 * k, sp),
-                 "adn_l1_norm")
-
   @property
   def groupable(self) -> bool:
     """SCALAR / VECTOR heads run in the grouped launch of the step (adn_head_group); MATRIX heads need their own
@@ -648,37 +643,47 @@ class EnsembleHead:
     return _lib.HeadBook(self.ema_state.data_ptr(), self.out3.data_ptr(), self._sub_loss_src.data_ptr(), self.trace.data_ptr(),
                          self.decay, self.trace_capacity)
 
-  def enqueue(self, labels, labels_f, step_dev, sp: int, xp: Optional[torch.Tensor] = None, bookkeeping: bool = True):
-    """steps 6-13 on pre-update values: ensemble logits, loss, penalty, mixture-weight gradient and update, EMA,
-    trace.  Uses only its own scratch, so it can run beside the backward waves.  bookkeeping=False leaves the
-    EMA / trace row / mixture-weight update to the step's grouped launches."""
+  def enqueue_matrix(self, labels, labels_f, sp: int, xp: torch.Tensor):
+    """steps 6-11 of a MATRIX head in the wave schedule, on pre-update values: the members' plane GEMMs and L1 norms,
+    ensemble logits, loss, penalty and the mixture-weight gradients.  Its EMA, trace row and update run in the
+    step's grouped launches."""
     lib, B, C = self.lib, self.batch, self.C
-    lab = labels.data_ptr() if labels is not None else None
-    labf = labels_f.data_ptr() if labels_f is not None else None
     train_ens = self.ens_opt is not None
-    matrix = self.mix == _lib.MIX_MATRIX
-    if matrix:
-      self.matrix_forward(xp, sp)
+    matrix_member_logits(lib, self.member_nets, self.mwp, self.mw_logits, xp, sp, self.mw, self.mw_l1)
     _lib.check(lib.adn_ensemble_head(
         self.head, self.mix, self._members, len(self.member_nets), self.mix_w.data_ptr(), self.bias.data_ptr(),
-        self._gammas, self.reg_is_zero, self.reg_multiplier, lab, labf, self.out3.data_ptr(),
-        self.d_mix_w.data_ptr() if (train_ens and not matrix) else None,
+        self._gammas, self.reg_is_zero, self.reg_multiplier, labels.data_ptr() if labels is not None else None,
+        labels_f.data_ptr() if labels_f is not None else None, self.out3.data_ptr(), None,
         self.d_bias.data_ptr() if (train_ens and self.ens.use_bias) else None,
-        self.dens.data_ptr() if (train_ens and matrix) else None, None, B, C, self.head_ws.data_ptr(),
-        self.head_ws_bytes, sp), "adn_ensemble_head")
-    if train_ens and matrix:
-      # dW_k = last_layer_k^T @ dLoss/d(ens)  + reg_multiplier * gamma_k * sign(W_k)   (weighted.py:606-617)
-      _lib.check(lib.adn_planes_split_scaled(self.dens.data_ptr(), B, C, self.densp.data_ptr(), self.dz_log2, sp),
-                 "adn_planes_split_scaled")
-      for k, m in enumerate(self.member_nets):
-        _lib.check(lib.adn_dense_bwd_p(m.last_layer_planes(xp).data_ptr(), None, self.densp.data_ptr(), None, None, None,
-                                       self.d_mw[k].data_ptr(), B, m.last_layer_dim, C, 0, self.dz_log2,
-                                       self.mw_ws.data_ptr(), self.mw_ws_bytes, sp), "adn_dense_bwd_p")
-        if not self.reg_is_zero:
-          _lib.check(lib.adn_l1_grad_add(self.d_mw[k].data_ptr(), self.mw[k].data_ptr(), self.mw[k].numel(),
-                                         self.reg_multiplier * self.gammas[k], sp), "adn_l1_grad_add")
-    if not bookkeeping:
+        self.dens.data_ptr() if train_ens else None, None, B, C, self.head_ws.data_ptr(), self.head_ws_bytes, sp),
+               "adn_ensemble_head")
+    if not train_ens:
       return
+    # dW_k = last_layer_k^T @ dLoss/d(ens)  + reg_multiplier * gamma_k * sign(W_k)   (weighted.py:606-617); each dW
+    # GEMM is launched alone: its split-K count, and so its bytes, depend on the group it runs in
+    _lib.check(lib.adn_planes_split_scaled(self.dens.data_ptr(), B, C, self.densp.data_ptr(), self.dz_log2, sp),
+               "adn_planes_split_scaled")
+    for k, m in enumerate(self.member_nets):
+      op = _lib.BwdOp(m.last_layer_planes(xp).data_ptr(), None, self.densp.data_ptr(), None, None, None,
+                      self.d_mw[k].data_ptr(), m.last_layer_dim, C, 0, self.dz_log2, self.mw_ws.data_ptr(),
+                      self.mw_ws_bytes, 0.0, 0.0)
+      _lib.check(lib.adn_dense_bwd_p_group((_lib.BwdOp * 1)(op), 1, B, sp), "adn_dense_bwd_p_group")
+      if not self.reg_is_zero:
+        _lib.check(lib.adn_l1_grad_add(self.d_mw[k].data_ptr(), self.mw[k].data_ptr(), self.mw[k].numel(),
+                                       self.reg_multiplier * self.gammas[k], sp), "adn_l1_grad_add")
+
+  def enqueue_simt(self, labels, labels_f, step_dev, sp: int):
+    """steps 6-13 of a SCALAR / VECTOR head on the SIMT cross-check path, on pre-update values: ensemble logits, loss,
+    penalty, mixture-weight gradient, EMA, trace row and mixture-weight update, op by op."""
+    lib = self.lib
+    train_ens = self.ens_opt is not None
+    _lib.check(lib.adn_ensemble_head(
+        self.head, self.mix, self._members, len(self.member_nets), self.mix_w.data_ptr(), self.bias.data_ptr(),
+        self._gammas, self.reg_is_zero, self.reg_multiplier, labels.data_ptr() if labels is not None else None,
+        labels_f.data_ptr() if labels_f is not None else None, self.out3.data_ptr(),
+        self.d_mix_w.data_ptr() if train_ens else None,
+        self.d_bias.data_ptr() if (train_ens and self.ens.use_bias) else None, None, None, self.batch, self.C,
+        self.head_ws.data_ptr(), self.head_ws_bytes, sp), "adn_ensemble_head")
     _lib.check(lib.adn_ema_update(self.ema_state.data_ptr(), self.out3.data_ptr() + 8, self.decay, sp),
                "adn_ema_update")
     _lib.check(lib.adn_record_scalars(self._trace_src, 4, self.trace.data_ptr(), 4, step_dev.data_ptr(),
@@ -693,7 +698,7 @@ class EnsembleHead:
     rows = self.batch if rows is None else rows
     _check_head_ws(rows, self.C, len(self.member_nets), self.head_ws_bytes)
     if self.mix == _lib.MIX_MATRIX:
-      self.matrix_forward(xp, sp)
+      matrix_member_logits(self.lib, self.member_nets, self.mwp, self.mw_logits, xp, sp, self.mw, self.mw_l1)
     _lib.check(self.lib.adn_ensemble_head(
         self.head, self.mix, self._members, len(self.member_nets), self.mix_w.data_ptr(), self.bias.data_ptr(),
         self._gammas, self.reg_is_zero, self.reg_multiplier,
@@ -784,15 +789,15 @@ class CandidatePlan:
       self.dzp_out = new_planes(batch, dims[-1], device)
       self.dzp = [new_planes(batch, hid, device) for _ in range(2)] if hid else []
       self.dz = []
-      ws_bytes = max(_lib.query(_lib.Q_DENSE_BWD_P_WS, batch, dims[i], dims[i + 1]) for i in range(len(dims) - 1))
-      ws_bytes = max(ws_bytes, _lib.query(_lib.Q_COLSUM_WS, batch, dims[-1]))
+      bwd_ws = max(_lib.query(_lib.Q_DENSE_BWD_P_WS, batch, dims[i], dims[i + 1]) for i in range(len(dims) - 1))
+      self.bwd_ws_bytes = max(bwd_ws, _lib.query(_lib.Q_COLSUM_WS, batch, dims[-1]))
+      self.bwd_ws = torch.empty((self.bwd_ws_bytes,), dtype=torch.uint8, device=device)
+      ws_bytes = 0                    # `workspace` serves the subnetwork's own head op alone
     else:
       self.dz = [torch.empty((batch, hid), **f32) for _ in range(2)] if hid else []
+      # `workspace` serves the backward and the subnetwork's own head loss, one after the other on its stream
       ws_bytes = max(_lib.query(_lib.Q_DENSE_BWD_WS, batch, dims[i], dims[i + 1]) for i in range(len(dims) - 1))
-    if self.planes:
-      self.bwd_ws_bytes = ws_bytes
-      self.bwd_ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=device)
-    ws_bytes = max(ws_bytes, _lib.query(_lib.Q_HEAD_WS, batch, logits_dim, 1))   # the subnetwork's own head loss
+    ws_bytes = max(ws_bytes, _lib.query(_lib.Q_HEAD_WS, batch, logits_dim, 1))
     self.workspace = torch.empty((ws_bytes,), dtype=torch.uint8, device=device)
     self.ws_bytes = ws_bytes
     self.sub_out3 = galloc((3,)).zero_()           # {loss, -, -} of the subnetwork's own head
@@ -806,7 +811,8 @@ class CandidatePlan:
       self.xp_own = None if self.net.stem else new_planes(batch, self.net.in_dim, device)
       self.labels_own = (torch.empty((batch,), dtype=torch.int64, device=device) if head == "softmax_xent"
                          else torch.empty((batch, logits_dim), **f32))
-      self.own_loss = torch.zeros((1,), **f32)    # loss on the bagged minibatch (not reported by the reference)
+      self.own_out3 = torch.zeros((3,), **f32)    # {loss, -, -} on the bagged minibatch (not reported by the reference)
+      self.own_loss = self.own_out3[:1]
     params, self._grads, planes = [], [], []
     if self.net.stem:
       # conv stem: dense gradient of the pooled features (first dense layer's dX), kernel / bias gradients
@@ -841,47 +847,25 @@ class CandidatePlan:
   trace_capacity = property(lambda self: self.ehead.trace_capacity)
   ens_opt = property(lambda self: self.ehead.ens_opt)
 
-  def enqueue_train_step(self, x: torch.Tensor, labels: torch.Tensor, labels_f: Optional[torch.Tensor],
-                         step_dev: torch.Tensor, sp: int, xp: Optional[torch.Tensor] = None):
-    """SURVEY.md section 3.3 steps 1-13 for this candidate (frozen logits already computed)."""
+  def enqueue_simt_step(self, x: torch.Tensor, labels: torch.Tensor, labels_f: Optional[torch.Tensor],
+                        step_dev: torch.Tensor, sp: int):
+    """SURVEY.md section 3.3 steps 1-13 for this candidate on the fp32 SIMT cross-check path, op by op on stream `sp`
+    (frozen logits already computed).  The plane path trains on the wave schedule (IterationPlan._enqueue_waves)."""
     lib, net, B, C = self.lib, self.net, self.batch, self.C
-    if net.stem:
-      raise NotImplementedError("conv-stem subnetworks train on the wave schedule (IterationPlan._enqueue_waves)")
     lab = labels.data_ptr() if labels is not None else None
     labf = labels_f.data_ptr() if labels_f is not None else None
     wsp = self.workspace.data_ptr()
     # steps 1-2: subnetwork forward
-    net.forward(lib, x, sp, xp)
-    # step 3: subnetwork loss + dlogits (plane path: also its split planes and column sums = db of the logits layer)
-    if self.planes:
-      _lib.check(lib.adn_head_loss_p(self.head, net.logits.data_ptr(), lab, labf, self.sub_loss.data_ptr(),
-                                     self.dlogits.data_ptr(), self.dzp_out.data_ptr(),
-                                     self.dbs[len(net.ws) - 1].data_ptr(), self.dz_log2, B, C, wsp, self.ws_bytes, sp),
-                 "adn_head_loss_p")
-    else:
-      _lib.check(lib.adn_head_loss(self.head, net.logits.data_ptr(), lab, labf, self.sub_loss.data_ptr(),
-                                   self.dlogits.data_ptr(), B, C, wsp, self.ws_bytes, sp), "adn_head_loss")
+    net.forward(lib, x, sp)
+    # step 3: subnetwork loss + dlogits
+    _lib.check(lib.adn_head_loss(self.head, net.logits.data_ptr(), lab, labf, self.sub_loss.data_ptr(),
+                                 self.dlogits.data_ptr(), B, C, wsp, self.ws_bytes, sp), "adn_head_loss")
     # steps 6-13: ensemble head on pre-update values, EMA, trace, mixture-weight update
     if self.has_head:
-      self.ehead.enqueue(labels, labels_f, step_dev, sp, xp)
+      self.ehead.enqueue_simt(labels, labels_f, step_dev, sp)
     # step 4: backward through the subnetwork's own variables only
-    n = len(net.ws)
-    if self.planes:
-      # one call per layer produces dW_i, the planes of dZ_{i-1} (ReLU mask = sign bits of h_{i-1}) and
-      # db_{i-1} = colsum(dZ_{i-1}); the planes of dlogits and db of the logits layer came from the head kernel
-      dzp = self.dzp_out
-      for i in range(n - 1, -1, -1):
-        xin = xp if i == 0 else net.hp[i - 1]
-        dxp = self.dzp[i % 2] if i > 0 else None
-        _lib.check(lib.adn_dense_bwd_p(xin.data_ptr(), net.wps[i].data_ptr(), dzp.data_ptr(),
-                                       dxp.data_ptr() if dxp is not None else None, None,
-                                       self.dbs[i - 1].data_ptr() if i > 0 else None, self.dws[i].data_ptr(), B,
-                                       net.dims[i], net.dims[i + 1], 1 if i > 0 else 0, self.dz_log2, wsp,
-                                       self.ws_bytes, sp),
-                   "adn_dense_bwd_p")
-        dzp = dxp
     dz = self.dlogits
-    for i in range(n - 1, -1, -1) if not self.planes else ():
+    for i in range(len(net.ws) - 1, -1, -1):
       xin = x if i == 0 else net.acts[i - 1]
       # dz ping-pong buffers are sized for the widest hidden layer; carve a contiguous [B, d_i] view
       dx = self.dz[i % 2].view(-1)[:B * net.dims[i]].view(B, net.dims[i]) if i > 0 else None
@@ -926,28 +910,15 @@ class CandidatePlan:
     self.x_own.copy_(torch.as_tensor(x).reshape(self.x_own.shape), non_blocking=True)
     self.labels_own.copy_(torch.as_tensor(y).reshape(self.labels_own.shape), non_blocking=True)
 
-  def enqueue_sub_loss(self, labels, labels_f, sp: int, loss_out: Optional[torch.Tensor] = None):
-    """step 3 after the forward waves: subnetwork loss, dlogits (dense + planes) and db of the logits layer."""
-    lab = labels.data_ptr() if labels is not None else None
-    labf = labels_f.data_ptr() if labels_f is not None else None
-    loss_out = loss_out if loss_out is not None else self.sub_loss
-    _lib.check(self.lib.adn_head_loss_p(self.head, self.net.logits.data_ptr(), lab, labf, loss_out.data_ptr(),
-                                        self.dlogits.data_ptr(), self.dzp_out.data_ptr(),
-                                        self.dbs[len(self.net.ws) - 1].data_ptr(), self.dz_log2, self.batch, self.C,
-                                        self.workspace.data_ptr(), self.ws_bytes, sp), "adn_head_loss_p")
-
-  def sub_head_op(self, labels, labels_f) -> "_lib.HeadOp":
-    """step 3 as an adn_head_op (colsum_only): subnetwork loss, dlogits (dense + scaled planes), db of the logits layer."""
+  def sub_head_op(self, labels, labels_f, out3: torch.Tensor) -> "_lib.HeadOp":
+    """step 3 as an adn_head_op (colsum_only): subnetwork loss into out3[0], dlogits (dense + scaled planes), db of the
+    logits layer."""
     return _lib.HeadOp(self.head, _lib.MIX_SCALAR, ctypes.cast(self._logits_ptr, ctypes.POINTER(ctypes.c_void_p)), 1, 1,
                        None, None, None, 1.0, self.dz_log2, labels.data_ptr() + self.row0 * 8 if labels is not None else None,
                        labels_f.data_ptr() + self.row0 * self.C * 4 if labels_f is not None else None,
-                       self.sub_out3.data_ptr(), None,
+                       out3.data_ptr(), None,
                        self.dbs[len(self.net.ws) - 1].data_ptr(), self.dlogits.data_ptr(), None, self.dzp_out.data_ptr(),
                        1, 0, self.workspace.data_ptr(), self.ws_bytes)
-
-  def enqueue_ensemble(self, labels, labels_f, step_dev, sp: int, xp: Optional[torch.Tensor] = None):
-    if self.has_head:
-      self.ehead.enqueue(labels, labels_f, step_dev, sp, xp)
 
   def bwd_op(self, k: int, xp: torch.Tensor) -> "_lib.BwdOp":
     """k-th backward wave = layer n-1-k: dW_i, planes of dZ_{i-1} (ReLU mask = sign bits of h_{i-1}) and
@@ -976,15 +947,6 @@ class CandidatePlan:
                                           self.d_stem_k.data_ptr(), self.d_stem_b.data_ptr(), self.batch, st["h"], st["w"],
                                           st["cin"], st["f"], self.stem_ws.data_ptr(), self.stem_ws_bytes, sp),
                "adn_conv_stem_bwd")
-
-  def enqueue_sub_update(self, sp: int):
-    self.sub_opt.apply(self.lib, self._grads, sp)
-
-  def enqueue_eval(self, x, labels, labels_f, ens_out: Optional[torch.Tensor], sp: int,
-                   xp: Optional[torch.Tensor] = None):
-    """Forward-only: subnetwork logits + ensemble logits/loss (evaluate / predict)."""
-    self.net.forward(self.lib, x, sp, xp)
-    self.ehead.enqueue_eval(labels, labels_f, ens_out, sp, xp)
 
 
 class IterationPlan:
@@ -1018,6 +980,9 @@ class IterationPlan:
     warm = lambda e: prev_ens_name is None or prev_ens_name == e.name
     shards = shards or {}
     for i in idx:
+      if i in shards and not planes_enabled():
+        # the SIMT step reads the minibatch from row 0 on and never averages the gradient arena
+        raise NotImplementedError("row-sharded candidates run on the plane path only")
       if i in shards and batch % shards[i].count != 0:
         raise ValueError("batch %d is not divisible by the %d row shards of candidate %d" % (batch, shards[i].count, i))
     self.candidates = [CandidatePlan(self.lib, s, self.frozen, ens, iteration,
@@ -1055,6 +1020,8 @@ class IterationPlan:
           own.has_head = True
           self.heads.append((gidx, own.ehead, local[0]))
           continue
+        if not planes_enabled():
+          raise NotImplementedError("ensembles that share subnetworks run on the plane path only")
         members = [self.frozen[i] for i in kidx] + [self.candidates[k].net for k in local]
         h = EnsembleHead(self.lib, full_name, members, len(kidx), e, batch, logits_dim,
                          head, adanet_loss_decay, trace_capacity, self.device,
@@ -1073,7 +1040,9 @@ class IterationPlan:
     self.trace_capacity = trace_capacity
     self.use_cuda_graph = use_cuda_graph
     self.multi_stream = multi_stream and len(self.candidates) > 1
-    self.streams = [torch.cuda.Stream(device=self.device) for _ in self.candidates] if self.multi_stream else []
+    # side streams of the SIMT schedule, one per candidate
+    self.streams = ([torch.cuda.Stream(device=self.device) for _ in self.candidates]
+                    if (self.multi_stream and self.xp is None) else [])
     self._graph = None
     self._warmed = False      # set by the first (eager) step
     self._stage = None
@@ -1121,11 +1090,32 @@ class IterationPlan:
     st["pending"] = False
 
   # -- one step --------------------------------------------------------------
+  def _fwd_waves(self, fwd, sp: int):
+    """Layer waves: one grouped forward launch per layer index and distinct batch size, larger batches first.
+    `fwd`: (net, input planes, batch, step counter of a TRAIN-mode forward or None, first minibatch row) per net."""
+    for w in range(max((len(n.ws) for n, _, _, _, _ in fwd), default=0)):
+      for bsz in sorted({b for _, _, b, _, _ in fwd}, reverse=True):
+        ops = [n.fwd_op(w, xp, sd, r0) for n, xp, b, sd, r0 in fwd if b == bsz and w < len(n.ws)]
+        if ops:
+          _lib.check(self.lib.adn_dense_fwd_p_group((_lib.FwdOp * len(ops))(*ops), len(ops), bsz, sp),
+                     "adn_dense_fwd_p_group")
+
+  def _bwd_waves(self, cands, xp_of, sp: int):
+    """Backward waves of the candidates, logits layer first: one grouped launch per wave and distinct batch size.
+    `xp_of(c)`: the input planes of candidate c."""
+    for k in range(max((len(c.net.ws) for c in cands), default=0)):
+      for bsz in sorted({c.batch for c in cands}, reverse=True):
+        ops = [c.bwd_op(k, xp_of(c)) for c in cands if c.batch == bsz and k < len(c.net.ws)]
+        if ops:
+          _lib.check(self.lib.adn_dense_bwd_p_group((_lib.BwdOp * len(ops))(*ops), len(ops), bsz, sp),
+                     "adn_dense_bwd_p_group")
+
   def _enqueue_waves(self):
     """Plane path: layer waves across ALL subnetworks of the GPU (frozen members and candidates) as grouped
     launches on the main stream; the per-candidate small work (losses, ensemble heads, EMA / trace rows, optimizers)
     is grouped into one launch each (22 launches per step for 8 candidates); row-sharded candidates average their
-    gradient arena across their ranks before the optimizer."""
+    gradient arena across their ranks before the optimizer.  Bagged subnetworks take their own step first, through
+    the same builders.  A rank without candidates only replays its frozen members."""
     lib = self.lib
     main = torch.cuda.current_stream(self.device)
     sp = main.cuda_stream
@@ -1139,22 +1129,16 @@ class IterationPlan:
                      "adn_planes_split")
         else:
           c.net.stem_forward(lib, c.x_own, sp)
-      for w in range(max(len(c.net.ws) for c in bag)):
-        ops = [c.net.fwd_op(w, c.xp_own, self.step_dev) for c in bag if w < len(c.net.ws)]
-        _lib.check(lib.adn_dense_fwd_p_group((_lib.FwdOp * len(ops))(*ops), len(ops), self.batch, sp),
-                   "adn_dense_fwd_p_group")
-      for c in bag:
-        lab_i = c.labels_own if self.labels is not None else None
-        lab_f = c.labels_own if self.labels is None else None
-        c.enqueue_sub_loss(lab_i, lab_f, sp, loss_out=c.own_loss)
-      for k in range(max(len(c.net.ws) for c in bag)):
-        ops = [c.bwd_op(k, c.xp_own) for c in bag if k < len(c.net.ws)]
-        _lib.check(lib.adn_dense_bwd_p_group((_lib.BwdOp * len(ops))(*ops), len(ops), self.batch, sp),
-                   "adn_dense_bwd_p_group")
+      self._fwd_waves([(c.net, c.xp_own, c.batch, self.step_dev, 0) for c in bag], sp)
+      own = self.labels is not None
+      ops = [c.sub_head_op(c.labels_own if own else None, None if own else c.labels_own, c.own_out3) for c in bag]
+      _lib.check(lib.adn_head_group((_lib.HeadOp * len(ops))(*ops), len(ops), self.batch, self.C, sp), "adn_head_group")
+      self._bwd_waves(bag, lambda c: c.xp_own, sp)
       for c in bag:
         if c.net.stem:
           c.enqueue_stem_bwd(c.x_own, sp)
-        c.enqueue_sub_update(sp)
+      oops = [c.sub_opt.op(c._grads) for c in bag]
+      _lib.check(lib.adn_opt_step_group((_lib.OptOp * len(oops))(*oops), len(oops), sp), "adn_opt_step_group")
     self._split_x(sp)
     # a row-sharded candidate consumes its own slice of the minibatch rows
     for c in self.sharded:
@@ -1169,33 +1153,23 @@ class IterationPlan:
     for c in self.candidates:
       if c.net.stem:
         c.net.stem_forward(lib, x_of(c), sp)
-    # layer waves: one grouped launch per wave and distinct batch size (whole candidates and frozen members run the
-    # full minibatch, row-sharded candidates their slice)
-    # candidates run in TRAIN mode (dropout); a row-sharded one draws its rows of the whole minibatch's mask
-    fwd = ([(f, self.xp, self.batch, None, 0) for f in self.frozen] +
-           [(c.net, xp_of(c), c.batch, self.step_dev, c.row0) for c in self.candidates])
-    for w in range(max(len(n.ws) for n, _, _, _, _ in fwd)):
-      for bsz in sorted({b for _, _, b, _, _ in fwd}, reverse=True):
-        ops = [n.fwd_op(w, xp, sd, r0) for n, xp, b, sd, r0 in fwd if b == bsz and w < len(n.ws)]
-        if ops:
-          _lib.check(lib.adn_dense_fwd_p_group((_lib.FwdOp * len(ops))(*ops), len(ops), bsz, sp), "adn_dense_fwd_p_group")
+    # whole candidates and frozen members run the full minibatch, row-sharded candidates their slice; candidates run
+    # in TRAIN mode (dropout), a row-sharded one draws its rows of the whole minibatch's mask
+    self._fwd_waves([(f, self.xp, self.batch, None, 0) for f in self.frozen] +
+                    [(c.net, xp_of(c), c.batch, self.step_dev, c.row0) for c in self.candidates], sp)
     # steps 3 and 6-11 of every candidate in one grouped launch (+ one finalize): the subnetwork losses (dlogits planes,
     # logits-layer bias gradients) and every SCALAR / VECTOR candidate-ensemble head; MATRIX heads run their plane
     # GEMMs around their own head launch
-    hops = [(c.sub_head_op(self.labels, self.labels_f), c.batch) for c in self.candidates]
+    hops = [(c.sub_head_op(self.labels, self.labels_f, c.sub_out3), c.batch) for c in self.candidates]
     hops += [(h.head_op(self.labels, self.labels_f), h.batch) for _, h, _ in self.heads if h.groupable]
     for bsz in sorted({b for _, b in hops}, reverse=True):
       ops = [o for o, b in hops if b == bsz]
       _lib.check(lib.adn_head_group((_lib.HeadOp * len(ops))(*ops), len(ops), bsz, self.C, sp), "adn_head_group")
     for _, h, _ in self.heads:
       if not h.groupable:
-        h.enqueue(self.labels, self.labels_f, self.step_dev, sp, self.xp, bookkeeping=False)
+        h.enqueue_matrix(self.labels, self.labels_f, sp, self.xp)
     trained = [c for c in self.candidates if not c.bagged]      # bagged subnetworks already took their step
-    for k in range(max([len(c.net.ws) for c in trained] or [0])):
-      for bsz in sorted({c.batch for c in trained}, reverse=True):
-        ops = [c.bwd_op(k, xp_of(c)) for c in trained if c.batch == bsz and k < len(c.net.ws)]
-        if ops:
-          _lib.check(lib.adn_dense_bwd_p_group((_lib.BwdOp * len(ops))(*ops), len(ops), bsz, sp), "adn_dense_bwd_p_group")
+    self._bwd_waves(trained, xp_of, sp)
     for c in trained:
       if c.net.stem:
         c.enqueue_stem_bwd(x_of(c), sp)
@@ -1218,26 +1192,24 @@ class IterationPlan:
     _lib.check(lib.adn_counter_add(self.step_dev.data_ptr(), 1, sp), "adn_counter_add")
 
   def _enqueue(self):
-    if self.xp is not None and self.candidates:
+    if self.xp is not None:
       return self._enqueue_waves()
+    # fp32 SIMT cross-check: the frozen members' forward, then every candidate's whole step op by op on its own stream
     lib = self.lib
     main = torch.cuda.current_stream(self.device)
     sp = main.cuda_stream
-    self._split_x(sp)
     for f in self.frozen:   # shared by every candidate ensemble on this GPU
-      f.forward(lib, self.x, sp, self.xp)
+      f.forward(lib, self.x, sp)
     if self.multi_stream:
       for c, s in zip(self.candidates, self.streams):
         s.wait_stream(main)
         with torch.cuda.stream(s):
-          c.enqueue_train_step(self.x, self.labels, self.labels_f, self.step_dev, s.cuda_stream, self.xp)
+          c.enqueue_simt_step(self.x, self.labels, self.labels_f, self.step_dev, s.cuda_stream)
       for s in self.streams:
         main.wait_stream(s)
     else:
       for c in self.candidates:
-        c.enqueue_train_step(self.x, self.labels, self.labels_f, self.step_dev, sp, self.xp)
-    if any(not any(h is c.ehead for c in self.candidates) for _, h, _ in self.heads):
-      raise NotImplementedError("ensembles that share subnetworks run on the plane path only")
+        c.enqueue_simt_step(self.x, self.labels, self.labels_f, self.step_dev, sp)
     _lib.check(lib.adn_counter_add(self.step_dev.data_ptr(), 1, sp), "adn_counter_add")
 
   def _split_x(self, sp: int):
@@ -1416,8 +1388,7 @@ class EnsembleEvalPlan:
     self.bias = torch.as_tensor(np.ascontiguousarray(bias, dtype=np.float32)).to(self.device)
     lam, beta = float(ens.adanet_lambda), float(ens.adanet_beta)
     self.reg_is_zero = int(lam == 0.0 and beta == 0.0)
-    self.gammas = [float(np.float32(beta) if lam == 0.0 else np.float32(np.float32(lam) * np.float32(m.complexity) + np.float32(beta)))
-                   for m in self.members]
+    self.gammas = gammas(lam, beta, [m.complexity for m in self.members])
     self._gammas = _lib.f32_array(self.gammas)
     self._members = _lib.ptr_array([t.data_ptr() for t in self.mw_logits] if self.mix == _lib.MIX_MATRIX
                                    else [m.logits.data_ptr() for m in self.members])
@@ -1446,10 +1417,7 @@ class EnsembleEvalPlan:
       for m in self.members:
         m.forward(self.lib, self.x, sp, self.xp)
       if self.mix == _lib.MIX_MATRIX:
-        for k, m in enumerate(self.members):
-          _lib.check(self.lib.adn_dense_fwd_p(m.last_layer_planes(self.xp).data_ptr(), self.mwp[k].data_ptr(), None, None,
-                                              self.mw_logits[k].data_ptr(), self.batch, m.last_layer_dim, self.C,
-                                              _lib.ACT_NONE, sp), "adn_dense_fwd_p")
+        matrix_member_logits(self.lib, self.members, self.mwp, self.mw_logits, self.xp, sp)
     _lib.check(self.lib.adn_ensemble_head(
         self.head, self.mix, self._members, len(self.members), self.mix_w.data_ptr(), self.bias.data_ptr(),
         self._gammas, self.reg_is_zero, 1.0, self.labels.data_ptr() if self.labels is not None else None,

@@ -214,6 +214,28 @@ def test_iteration_parity(built_lib, name, path):
 
 
 @pytest.mark.gpu
+@pytest.mark.parametrize("case", ["shared_heads", "shards"])
+def test_simt_refuses_at_construction(built_lib, case):
+  """The fp32 cross-check path trains each candidate with its own `*_grow` head on the whole minibatch: heads that
+  share subnetworks (here an AllStrategy ensemble) and row-sharded candidates are refused when the plan is built,
+  before any kernel has run or any state has changed."""
+  from adanet_b200 import _lib
+  from adanet_b200.core import engine as eng
+  specs = pu.make_specs([(1, 16), (2, 16)], 8, 3, 0, ("sgd", 0.01))[1]
+  kw = (dict(ensemble_candidates=[(0, "all", [0, 1], True)]) if case == "shared_heads"
+        else dict(shards={1: eng.ShardComm([0, 1], 0, None)}))
+  _lib.set_dense_path(_lib.PATH_SIMT)
+  try:
+    eng._require_cuda()
+    before = _lib.launch_count()
+    with pytest.raises(NotImplementedError, match="plane path only"):
+      eng.IterationPlan(0, specs, [], eng.EnsemblerPlanSpec(**ENS), 32, 8, 3, **kw)
+    assert _lib.launch_count() == before
+  finally:
+    _lib.set_dense_path(_lib.PATH_AUTO)
+
+
+@pytest.mark.gpu
 def test_bench_workload_parity_full_batch(built_lib):
   """bench.py's configuration itself (BASELINE configs[2]: 8 candidates 100->H->H->10, H in 64..1024, B=32768, SGD .05 /
   mixture SGD .01, lambda .01, beta .001) against the oracle: per-step losses of every candidate within 1e-5 and
