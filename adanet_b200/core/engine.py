@@ -24,8 +24,8 @@ builder per stage:
 
 With ADN_DENSE_PATH=simt the fp32 CUDA-core ABI is used instead, as an on-device
 cross-check: each candidate runs its whole step op by op (adn_dense_fwd /
-adn_head_loss / adn_ensemble_head / adn_dense_bwd / adn_opt_step) on its own
-stream (CandidatePlan.enqueue_simt_step).
+one-op adn_head_group calls of the same head op builders / adn_dense_bwd /
+adn_opt_step) on its own stream (CandidatePlan.enqueue_simt_step).
 
 Once shapes are fixed the whole step is captured in a CUDA graph, so a step is
 one graph launch.  PyTorch is used for device memory, streams and graphs only.
@@ -74,6 +74,11 @@ def _check_head_ws(rows: int, logits_dim: int, n_members: int, have: int):
   need = _lib.query(_lib.Q_HEAD_WS, rows, logits_dim, n_members)
   if need > have:
     raise RuntimeError("head workspace of %d bytes is too small for %d rows (needs %d)" % (have, rows, need))
+
+
+def _run_head(lib, op: "_lib.HeadOp", rows: int, dim: int, sp: int):
+  """One head op on its own: a one-op adn_head_group over `rows` examples."""
+  _lib.check(lib.adn_head_group((_lib.HeadOp * 1)(op), 1, rows, dim, sp), "adn_head_group")
 
 
 def _load_rows(x_buf: torch.Tensor, labels_buf: Optional[torch.Tensor], x, y) -> int:
@@ -626,16 +631,21 @@ class EnsembleHead:
     plane GEMMs around the head kernel."""
     return self.mix != _lib.MIX_MATRIX
 
-  def head_op(self, labels, labels_f) -> "_lib.HeadOp":
-    """This head as an adn_head_op: ensemble logits, loss, penalty, mixture-weight / bias gradients (steps 6-11)."""
-    train_ens = self.ens_opt is not None
+  def head_op(self, labels, labels_f, grads: bool = True, ens_out: Optional[torch.Tensor] = None) -> "_lib.HeadOp":
+    """This head as an adn_head_op: ensemble logits (into `ens_out` if given), loss and penalty (steps 6-10), and with
+    `grads` the gradients of a trained ensembler (step 11): mixture weights and bias, or for a MATRIX head its bias
+    and dLoss/d(ens), from which its weight gradients are GEMMs."""
+    train = grads and self.ens_opt is not None
+    matrix = self.mix == _lib.MIX_MATRIX
     return _lib.HeadOp(self.head, self.mix, ctypes.cast(self._members, ctypes.POINTER(ctypes.c_void_p)),
                        len(self.member_nets), self.reg_is_zero, self.mix_w.data_ptr(), self.bias.data_ptr(),
                        ctypes.cast(self._gammas, ctypes.POINTER(ctypes.c_float)), self.reg_multiplier, 0,
                        labels.data_ptr() + self.row0 * 8 if labels is not None else None,
                        labels_f.data_ptr() + self.row0 * self.C * 4 if labels_f is not None else None, self.out3.data_ptr(),
-                       self.d_mix_w.data_ptr() if train_ens else None,
-                       self.d_bias.data_ptr() if (train_ens and self.ens.use_bias) else None, None, None, None, 0, 0,
+                       self.d_mix_w.data_ptr() if (train and not matrix) else None,
+                       self.d_bias.data_ptr() if (train and self.ens.use_bias) else None,
+                       self.dens.data_ptr() if (train and matrix) else None,
+                       ens_out.data_ptr() if ens_out is not None else None, None, 0, 0,
                        self.head_ws.data_ptr(), self.head_ws_bytes)
 
   def book(self) -> "_lib.HeadBook":
@@ -648,16 +658,9 @@ class EnsembleHead:
     ensemble logits, loss, penalty and the mixture-weight gradients.  Its EMA, trace row and update run in the
     step's grouped launches."""
     lib, B, C = self.lib, self.batch, self.C
-    train_ens = self.ens_opt is not None
     matrix_member_logits(lib, self.member_nets, self.mwp, self.mw_logits, xp, sp, self.mw, self.mw_l1)
-    _lib.check(lib.adn_ensemble_head(
-        self.head, self.mix, self._members, len(self.member_nets), self.mix_w.data_ptr(), self.bias.data_ptr(),
-        self._gammas, self.reg_is_zero, self.reg_multiplier, labels.data_ptr() if labels is not None else None,
-        labels_f.data_ptr() if labels_f is not None else None, self.out3.data_ptr(), None,
-        self.d_bias.data_ptr() if (train_ens and self.ens.use_bias) else None,
-        self.dens.data_ptr() if train_ens else None, None, B, C, self.head_ws.data_ptr(), self.head_ws_bytes, sp),
-               "adn_ensemble_head")
-    if not train_ens:
+    _run_head(lib, self.head_op(labels, labels_f), B, C, sp)
+    if self.ens_opt is None:
       return
     # dW_k = last_layer_k^T @ dLoss/d(ens)  + reg_multiplier * gamma_k * sign(W_k)   (weighted.py:606-617); each dW
     # GEMM is launched alone: its split-K count, and so its bytes, depend on the group it runs in
@@ -676,19 +679,12 @@ class EnsembleHead:
     """steps 6-13 of a SCALAR / VECTOR head on the SIMT cross-check path, on pre-update values: ensemble logits, loss,
     penalty, mixture-weight gradient, EMA, trace row and mixture-weight update, op by op."""
     lib = self.lib
-    train_ens = self.ens_opt is not None
-    _lib.check(lib.adn_ensemble_head(
-        self.head, self.mix, self._members, len(self.member_nets), self.mix_w.data_ptr(), self.bias.data_ptr(),
-        self._gammas, self.reg_is_zero, self.reg_multiplier, labels.data_ptr() if labels is not None else None,
-        labels_f.data_ptr() if labels_f is not None else None, self.out3.data_ptr(),
-        self.d_mix_w.data_ptr() if train_ens else None,
-        self.d_bias.data_ptr() if (train_ens and self.ens.use_bias) else None, None, None, self.batch, self.C,
-        self.head_ws.data_ptr(), self.head_ws_bytes, sp), "adn_ensemble_head")
+    _run_head(lib, self.head_op(labels, labels_f), self.batch, self.C, sp)
     _lib.check(lib.adn_ema_update(self.ema_state.data_ptr(), self.out3.data_ptr() + 8, self.decay, sp),
                "adn_ema_update")
     _lib.check(lib.adn_record_scalars(self._trace_src, 4, self.trace.data_ptr(), 4, step_dev.data_ptr(),
                                       self.trace_capacity, sp), "adn_record_scalars")
-    if train_ens:
+    if self.ens_opt is not None:
       self.ens_opt.apply(lib, self._ens_grads, sp)
 
   def enqueue_eval(self, labels, labels_f, ens_out: Optional[torch.Tensor], sp: int, xp: Optional[torch.Tensor] = None,
@@ -699,12 +695,7 @@ class EnsembleHead:
     _check_head_ws(rows, self.C, len(self.member_nets), self.head_ws_bytes)
     if self.mix == _lib.MIX_MATRIX:
       matrix_member_logits(self.lib, self.member_nets, self.mwp, self.mw_logits, xp, sp, self.mw, self.mw_l1)
-    _lib.check(self.lib.adn_ensemble_head(
-        self.head, self.mix, self._members, len(self.member_nets), self.mix_w.data_ptr(), self.bias.data_ptr(),
-        self._gammas, self.reg_is_zero, self.reg_multiplier,
-        labels.data_ptr() if labels is not None else None, labels_f.data_ptr() if labels_f is not None else None,
-        self.out3.data_ptr(), None, None, None, ens_out.data_ptr() if ens_out is not None else None, rows,
-        self.C, self.head_ws.data_ptr(), self.head_ws_bytes, sp), "adn_ensemble_head")
+    _run_head(self.lib, self.head_op(labels, labels_f, grads=False, ens_out=ens_out), rows, self.C, sp)
 
   def mixture_weight_tensors(self) -> List[torch.Tensor]:
     """The trained mixture weights as tensors: [w] (SCALAR [N] / VECTOR [N,C]) or the N matrices (MATRIX)."""
@@ -852,14 +843,11 @@ class CandidatePlan:
     """SURVEY.md section 3.3 steps 1-13 for this candidate on the fp32 SIMT cross-check path, op by op on stream `sp`
     (frozen logits already computed).  The plane path trains on the wave schedule (IterationPlan._enqueue_waves)."""
     lib, net, B, C = self.lib, self.net, self.batch, self.C
-    lab = labels.data_ptr() if labels is not None else None
-    labf = labels_f.data_ptr() if labels_f is not None else None
     wsp = self.workspace.data_ptr()
     # steps 1-2: subnetwork forward
     net.forward(lib, x, sp)
     # step 3: subnetwork loss + dlogits
-    _lib.check(lib.adn_head_loss(self.head, net.logits.data_ptr(), lab, labf, self.sub_loss.data_ptr(),
-                                 self.dlogits.data_ptr(), B, C, wsp, self.ws_bytes, sp), "adn_head_loss")
+    _run_head(lib, self.sub_head_op(labels, labels_f, self.sub_out3), B, C, sp)
     # steps 6-13: ensemble head on pre-update values, EMA, trace, mixture-weight update
     if self.has_head:
       self.ehead.enqueue_simt(labels, labels_f, step_dev, sp)
@@ -911,14 +899,14 @@ class CandidatePlan:
     self.labels_own.copy_(torch.as_tensor(y).reshape(self.labels_own.shape), non_blocking=True)
 
   def sub_head_op(self, labels, labels_f, out3: torch.Tensor) -> "_lib.HeadOp":
-    """step 3 as an adn_head_op (colsum_only): subnetwork loss into out3[0], dlogits (dense + scaled planes), db of the
-    logits layer."""
+    """step 3 as an adn_head_op (colsum_only): subnetwork loss into out3[0] and dlogits; on the plane path also its
+    scaled planes and db of the logits layer (the SIMT backward forms db itself)."""
     return _lib.HeadOp(self.head, _lib.MIX_SCALAR, ctypes.cast(self._logits_ptr, ctypes.POINTER(ctypes.c_void_p)), 1, 1,
                        None, None, None, 1.0, self.dz_log2, labels.data_ptr() + self.row0 * 8 if labels is not None else None,
                        labels_f.data_ptr() + self.row0 * self.C * 4 if labels_f is not None else None,
                        out3.data_ptr(), None,
-                       self.dbs[len(self.net.ws) - 1].data_ptr(), self.dlogits.data_ptr(), None, self.dzp_out.data_ptr(),
-                       1, 0, self.workspace.data_ptr(), self.ws_bytes)
+                       self.dbs[len(self.net.ws) - 1].data_ptr() if self.planes else None, self.dlogits.data_ptr(), None,
+                       self.dzp_out.data_ptr() if self.planes else None, 1, 0, self.workspace.data_ptr(), self.ws_bytes)
 
   def bwd_op(self, k: int, xp: torch.Tensor) -> "_lib.BwdOp":
     """k-th backward wave = layer n-1-k: dW_i, planes of dZ_{i-1} (ReLU mask = sign bits of h_{i-1}) and
@@ -1355,7 +1343,7 @@ class IterationPlan:
 class EnsembleEvalPlan:
   """Forward-only evaluation of a finished ensemble (evaluate / predict and the
   `previous_ensemble` candidate of the Evaluator): frozen members replayed with
-  adn_dense_fwd, then adn_ensemble_head for logits and loss
+  adn_dense_fwd, then a one-op adn_head_group for logits and loss
   (adanet/core/estimator.py:1785-1882 rebuilds the same thing as a TF graph)."""
 
   def __init__(self, members: Sequence[DenseNet], mix_w: np.ndarray, bias: np.ndarray, ens: EnsemblerPlanSpec,
@@ -1418,12 +1406,13 @@ class EnsembleEvalPlan:
         m.forward(self.lib, self.x, sp, self.xp)
       if self.mix == _lib.MIX_MATRIX:
         matrix_member_logits(self.lib, self.members, self.mwp, self.mw_logits, self.xp, sp)
-    _lib.check(self.lib.adn_ensemble_head(
-        self.head, self.mix, self._members, len(self.members), self.mix_w.data_ptr(), self.bias.data_ptr(),
-        self._gammas, self.reg_is_zero, 1.0, self.labels.data_ptr() if self.labels is not None else None,
-        self.labels_f.data_ptr() if self.labels_f is not None else None, self.out3.data_ptr(), None, None, None,
-        self.ens_logits.data_ptr(), b, self.C, self.workspace.data_ptr(), self.ws_bytes, sp),
-               "adn_ensemble_head")
+    op = _lib.HeadOp(self.head, self.mix, ctypes.cast(self._members, ctypes.POINTER(ctypes.c_void_p)), len(self.members),
+                     self.reg_is_zero, self.mix_w.data_ptr(), self.bias.data_ptr(),
+                     ctypes.cast(self._gammas, ctypes.POINTER(ctypes.c_float)), 1.0, 0,
+                     self.labels.data_ptr() if self.labels is not None else None,
+                     self.labels_f.data_ptr() if self.labels_f is not None else None, self.out3.data_ptr(), None, None,
+                     None, self.ens_logits.data_ptr(), None, 0, 0, self.workspace.data_ptr(), self.ws_bytes)
+    _run_head(self.lib, op, b, self.C, sp)
     o = self.out3.cpu().numpy()
     return float(o[0]), float(o[1]), float(o[2])
 

@@ -54,7 +54,6 @@ int dense_path() {
 
 int64_t head_workspace_bytes_public(int64_t batch, int64_t dim, int64_t members);
 int heads_init();
-int heads_group_init();
 
 }  // namespace adn
 
@@ -66,8 +65,6 @@ extern "C" int adn_init(void) {
   static std::atomic<int> done{0};
   if (done.load()) return ADN_OK;
   int rc = heads_init();
-  if (rc) return rc;
-  rc = heads_group_init();
   if (rc) return rc;
   rc = pl::init();
   if (rc) return rc;
@@ -191,26 +188,66 @@ extern "C" int adn_planes_merge(const void* planes, int64_t rows, int64_t cols, 
   return pl::merge(pl::format(), planes, rows, cols, dst, as_stream(stream));
 }
 
+// Checks one forward op (`what` names it in messages) and fills its launch parameters; `srcs` receives its pieces.
+static int check_fwd_op(const adn_fwd_op& op, int64_t batch, const char* what, pl::FwdOp& o, pl::FwdSrc* srcs) {
+  if (!op.xp || !op.wp) return fail(ADN_ERR_INVALID, "%s: null pointer", what);
+  const int ns = op.n_srcs;
+  if (ns < 0 || ns > ADN_FWD_MAX_SRCS || (ns > 0 && !op.srcs))
+    return fail(ADN_ERR_INVALID, "%s: n_srcs %d (0..%d, srcs non-NULL)", what, ns, ADN_FWD_MAX_SRCS);
+  int64_t k_total = op.in;
+  for (int q = 0; q < ns; ++q) {
+    const adn_fwd_src& s = op.srcs[q];
+    if (!s.xp || !s.wp) return fail(ADN_ERR_INVALID, "%s: piece %d: null pointer", what, q);
+    if (bad_shape(batch, s.in, op.out))
+      return fail(ADN_ERR_INVALID, "%s: piece %d: bad shape (in %lld)", what, q, (long long)s.in);
+    if (!pl::planes_aligned(s.xp) || !pl::planes_aligned(s.wp))
+      return fail(ADN_ERR_INVALID, "%s: piece %d: plane buffers must be 256 B aligned", what, q);
+    srcs[q] = pl::FwdSrc{s.xp, s.wp, s.in};
+    k_total += s.in;
+  }
+  if (ns > 0 && k_total > INT32_MAX) return fail(ADN_ERR_INVALID, "%s: total K too large", what);
+  if ((op.yp == nullptr) == (op.y == nullptr)) return fail(ADN_ERR_INVALID, "%s: exactly one of yp / y", what);
+  if (bad_shape(batch, op.in, op.out)) return fail(ADN_ERR_INVALID, "%s: bad shape", what);
+  if (op.act != ADN_ACT_NONE && op.act != ADN_ACT_RELU) return fail(ADN_ERR_INVALID, "%s: bad act %d", what, op.act);
+  if (op.dropout_rate != 0.f) {
+    if (!(op.dropout_rate > 0.f && op.dropout_rate < 1.f) || !op.yp || !op.dropout_step_dev)
+      return fail(ADN_ERR_INVALID, "%s: dropout needs 0 < rate < 1, planes out and a step counter", what);
+    if (op.dropout_row0 < 0) return fail(ADN_ERR_INVALID, "%s: dropout_row0 < 0", what);
+  }
+  // the dropout fields are read only when dropout_rate > 0
+  o = pl::FwdOp{op.xp, op.wp, op.bias, op.yp, op.y, op.in, op.out, op.act, op.dropout_rate, op.dropout_seed,
+                op.dropout_layer, op.dropout_row0, op.dropout_step_dev, ns > 0 ? srcs : nullptr, ns};
+  return ADN_OK;
+}
+
+// Checks one backward op (`what` names it in messages) and fills its launch parameters.
+static int check_bwd_op(const adn_bwd_op& p, int64_t batch, const char* what, pl::BwdOp& o) {
+  if (!p.xp || !p.dzp || !p.workspace) return fail(ADN_ERR_INVALID, "%s: null pointer", what);
+  if ((p.dxp || p.dx) && !p.wp) return fail(ADN_ERR_INVALID, "%s: wp required for dx", what);
+  if (p.dxp && p.dx) return fail(ADN_ERR_INVALID, "%s: at most one of dxp / dx", what);
+  if (p.dx_colsum && !(p.dxp || p.dx)) return fail(ADN_ERR_INVALID, "%s: dx_colsum needs dx", what);
+  if (bad_shape(batch, p.in, p.out)) return fail(ADN_ERR_INVALID, "%s: bad shape", what);
+  if (p.dz_log2_scale < -60 || p.dz_log2_scale > 60) return fail(ADN_ERR_INVALID, "%s: bad dz_log2_scale", what);
+  o = pl::BwdOp{p.xp, p.wp, p.dzp, p.dxp, p.dx, p.dx_colsum, p.dw, p.in, p.out, p.x_relu_mask, p.dz_log2_scale,
+                p.workspace, p.workspace_bytes};
+  if (p.dx_mul != 0.f) o.dx_mul = p.dx_mul;
+  return ADN_OK;
+}
+
 extern "C" int adn_dense_fwd_p(const void* xp, const void* wp, const float* b, void* yp, float* y, int64_t batch,
                                int64_t in, int64_t out, int act, void* stream) {
-  if (!xp || !wp) return fail(ADN_ERR_INVALID, "adn_dense_fwd_p: null pointer");
-  if ((yp == nullptr) == (y == nullptr)) return fail(ADN_ERR_INVALID, "adn_dense_fwd_p: exactly one of yp / y");
-  if (bad_shape(batch, in, out)) return fail(ADN_ERR_INVALID, "adn_dense_fwd_p: bad shape");
-  if (act != ADN_ACT_NONE && act != ADN_ACT_RELU) return fail(ADN_ERR_INVALID, "adn_dense_fwd_p: bad act %d", act);
-  return pl::dense_fwd(pl::format(), xp, wp, b, yp, y, batch, in, out, act, as_stream(stream));
+  pl::FwdOp o;
+  const int rc = check_fwd_op(adn_fwd_op{xp, wp, b, yp, y, in, out, act}, batch, "adn_dense_fwd_p", o, nullptr);
+  return rc ? rc : pl::dense_fwd_group(pl::format(), &o, 1, batch, as_stream(stream));
 }
 
 extern "C" int adn_dense_bwd_p(const void* xp, const void* wp, const void* dzp, void* dxp, float* dx,
                                float* dx_colsum, float* dw, int64_t batch, int64_t in, int64_t out, int x_relu_mask,
                                int dz_log2_scale, void* workspace, int64_t workspace_bytes, void* stream) {
-  if (!xp || !dzp || !workspace) return fail(ADN_ERR_INVALID, "adn_dense_bwd_p: null pointer");
-  if ((dxp || dx) && !wp) return fail(ADN_ERR_INVALID, "adn_dense_bwd_p: wp required when dx requested");
-  if (dxp && dx) return fail(ADN_ERR_INVALID, "adn_dense_bwd_p: at most one of dxp / dx");
-  if (dx_colsum && !(dxp || dx)) return fail(ADN_ERR_INVALID, "adn_dense_bwd_p: dx_colsum needs dx");
-  if (bad_shape(batch, in, out)) return fail(ADN_ERR_INVALID, "adn_dense_bwd_p: bad shape");
-  if (dz_log2_scale < -60 || dz_log2_scale > 60) return fail(ADN_ERR_INVALID, "adn_dense_bwd_p: bad dz_log2_scale");
-  return pl::dense_bwd(pl::format(), xp, wp, dzp, dxp, dx, dx_colsum, dw, batch, in, out, x_relu_mask, dz_log2_scale,
-                       workspace, workspace_bytes, as_stream(stream));
+  const adn_bwd_op op{xp, wp, dzp, dxp, dx, dx_colsum, dw, in, out, x_relu_mask, dz_log2_scale, workspace, workspace_bytes};
+  pl::BwdOp o;
+  const int rc = check_bwd_op(op, batch, "adn_dense_bwd_p", o);
+  return rc ? rc : pl::dense_bwd_group(pl::format(), &o, 1, batch, as_stream(stream));
 }
 
 extern "C" int adn_colsum(const float* x, int64_t rows, int64_t cols, float* out, void* workspace,
@@ -219,7 +256,8 @@ extern "C" int adn_colsum(const float* x, int64_t rows, int64_t cols, float* out
   if (bad_shape(rows, cols, 1)) return fail(ADN_ERR_INVALID, "adn_colsum: bad shape");
   if (workspace_bytes < 64 * cols * (int64_t)sizeof(float))
     return fail(ADN_ERR_WORKSPACE, "adn_colsum: workspace too small");
-  return simt::colsum(x, out, rows, cols, reinterpret_cast<float*>(workspace), as_stream(stream));
+  const simt::ColsumJob job{x, out, rows, cols, reinterpret_cast<float*>(workspace)};
+  return simt::colsum_group(&job, 1, as_stream(stream));
 }
 
 extern "C" int adn_dense_fwd_p_group(const adn_fwd_op* ops, int n, int64_t batch, void* stream) {
@@ -228,42 +266,9 @@ extern "C" int adn_dense_fwd_p_group(const adn_fwd_op* ops, int n, int64_t batch
   pl::FwdOp o[256];
   pl::FwdSrc srcs[256][ADN_FWD_MAX_SRCS];
   for (int i = 0; i < n; ++i) {
-    if (!ops[i].xp || !ops[i].wp) return fail(ADN_ERR_INVALID, "adn_dense_fwd_p_group: op %d: null pointer", i);
-    const int ns = ops[i].n_srcs;
-    if (ns < 0 || ns > ADN_FWD_MAX_SRCS || (ns > 0 && !ops[i].srcs))
-      return fail(ADN_ERR_INVALID, "adn_dense_fwd_p_group: op %d: n_srcs %d (0..%d, srcs non-NULL)", i, ns, ADN_FWD_MAX_SRCS);
-    int64_t k_total = ops[i].in;
-    for (int q = 0; q < ns; ++q) {
-      const adn_fwd_src& s = ops[i].srcs[q];
-      if (!s.xp || !s.wp) return fail(ADN_ERR_INVALID, "adn_dense_fwd_p_group: op %d: piece %d: null pointer", i, q);
-      if (bad_shape(batch, s.in, ops[i].out))
-        return fail(ADN_ERR_INVALID, "adn_dense_fwd_p_group: op %d: piece %d: bad shape (in %lld)", i, q, (long long)s.in);
-      if (!pl::planes_aligned(s.xp) || !pl::planes_aligned(s.wp))
-        return fail(ADN_ERR_INVALID, "adn_dense_fwd_p_group: op %d: piece %d: plane buffers must be 256 B aligned", i, q);
-      srcs[i][q] = pl::FwdSrc{s.xp, s.wp, s.in};
-      k_total += s.in;
-    }
-    if (ns > 0 && k_total > INT32_MAX) return fail(ADN_ERR_INVALID, "adn_dense_fwd_p_group: op %d: total K too large", i);
-    if ((ops[i].yp == nullptr) == (ops[i].y == nullptr))
-      return fail(ADN_ERR_INVALID, "adn_dense_fwd_p_group: op %d: exactly one of yp / y", i);
-    if (bad_shape(batch, ops[i].in, ops[i].out)) return fail(ADN_ERR_INVALID, "adn_dense_fwd_p_group: op %d: bad shape", i);
-    if (ops[i].act != ADN_ACT_NONE && ops[i].act != ADN_ACT_RELU)
-      return fail(ADN_ERR_INVALID, "adn_dense_fwd_p_group: op %d: bad act %d", i, ops[i].act);
-    o[i] = pl::FwdOp{ops[i].xp, ops[i].wp, ops[i].bias, ops[i].yp, ops[i].y, ops[i].in, ops[i].out, ops[i].act};
-    if (ns > 0) {
-      o[i].srcs = srcs[i];
-      o[i].n_srcs = ns;
-    }
-    if (ops[i].dropout_rate != 0.f) {
-      if (!(ops[i].dropout_rate > 0.f && ops[i].dropout_rate < 1.f) || !ops[i].yp || !ops[i].dropout_step_dev)
-        return fail(ADN_ERR_INVALID, "adn_dense_fwd_p_group: op %d: dropout needs 0 < rate < 1, planes out and a step counter", i);
-      if (ops[i].dropout_row0 < 0) return fail(ADN_ERR_INVALID, "adn_dense_fwd_p_group: op %d: dropout_row0 < 0", i);
-      o[i].dropout_row0 = ops[i].dropout_row0;
-      o[i].dropout_rate = ops[i].dropout_rate;
-      o[i].dropout_seed = ops[i].dropout_seed;
-      o[i].dropout_layer = ops[i].dropout_layer;
-      o[i].dropout_step = ops[i].dropout_step_dev;
-    }
+    char what[48];
+    snprintf(what, sizeof(what), "adn_dense_fwd_p_group: op %d", i);
+    if (const int rc = check_fwd_op(ops[i], batch, what, o[i], srcs[i])) return rc;
   }
   return pl::dense_fwd_group(pl::format(), o, n, batch, as_stream(stream));
 }
@@ -273,17 +278,9 @@ extern "C" int adn_dense_bwd_p_group(const adn_bwd_op* ops, int n, int64_t batch
   if (n > 256) return fail(ADN_ERR_UNSUPPORTED, "adn_dense_bwd_p_group: n %d > 256", n);
   pl::BwdOp o[256];
   for (int i = 0; i < n; ++i) {
-    const adn_bwd_op& p = ops[i];
-    if (!p.xp || !p.dzp || !p.workspace) return fail(ADN_ERR_INVALID, "adn_dense_bwd_p_group: op %d: null pointer", i);
-    if ((p.dxp || p.dx) && !p.wp) return fail(ADN_ERR_INVALID, "adn_dense_bwd_p_group: op %d: wp required for dx", i);
-    if (p.dxp && p.dx) return fail(ADN_ERR_INVALID, "adn_dense_bwd_p_group: op %d: at most one of dxp / dx", i);
-    if (p.dx_colsum && !(p.dxp || p.dx)) return fail(ADN_ERR_INVALID, "adn_dense_bwd_p_group: op %d: dx_colsum needs dx", i);
-    if (bad_shape(batch, p.in, p.out)) return fail(ADN_ERR_INVALID, "adn_dense_bwd_p_group: op %d: bad shape", i);
-    if (p.dz_log2_scale < -60 || p.dz_log2_scale > 60)
-      return fail(ADN_ERR_INVALID, "adn_dense_bwd_p_group: op %d: bad dz_log2_scale", i);
-    o[i] = pl::BwdOp{p.xp, p.wp, p.dzp, p.dxp, p.dx, p.dx_colsum, p.dw, p.in, p.out, p.x_relu_mask, p.dz_log2_scale,
-                     p.workspace, p.workspace_bytes};
-    if (p.dx_mul != 0.f) o[i].dx_mul = p.dx_mul;
+    char what[48];
+    snprintf(what, sizeof(what), "adn_dense_bwd_p_group: op %d", i);
+    if (const int rc = check_bwd_op(ops[i], batch, what, o[i])) return rc;
   }
   return pl::dense_bwd_group(pl::format(), o, n, batch, as_stream(stream));
 }

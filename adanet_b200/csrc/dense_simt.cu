@@ -6,36 +6,6 @@
 namespace adn {
 namespace simt {
 
-static __global__ void reduce_partials_kernel(const float* __restrict__ part, float* __restrict__ out,
-                                       int64_t n, int S, int64_t stride) {
-  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  float acc = 0.f;
-  for (int s = 0; s < S; ++s) acc += part[(size_t)s * stride + i];
-  out[i] = acc;
-}
-
-static __global__ void __launch_bounds__(256)
-colsum_partial_kernel(const float* __restrict__ dz, float* __restrict__ part, int rows, int N,
-                      int rows_per_slice) {
-  __shared__ float sm[8][33];
-  const int cx = threadIdx.x % 32, ry = threadIdx.x / 32;
-  const int n = blockIdx.x * 32 + cx;
-  const int r0 = blockIdx.y * rows_per_slice;
-  const int r1 = min(rows, r0 + rows_per_slice);
-  float acc = 0.f;
-  if (n < N)
-    for (int r = r0 + ry; r < r1; r += 8) acc += dz[(size_t)r * N + n];
-  sm[ry][cx] = acc;
-  __syncthreads();
-  if (ry == 0 && n < N) {
-    float t = 0.f;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) t += sm[i][cx];
-    part[(size_t)blockIdx.y * N + n] = t;
-  }
-}
-
 // rows per first-level slice: at most 64 slices, at least 64 rows each (each thread then adds >= 8 rows)
 static inline int colsum_slice_rows(int64_t rows) {
   int64_t r = ceil_div(rows, 64);
@@ -43,22 +13,7 @@ static inline int colsum_slice_rows(int64_t rows) {
   return (int)(r < 64 ? 64 : r);
 }
 
-int reduce_partials(const float* part, float* out, int64_t n, int S, int64_t stride, cudaStream_t st) {
-  reduce_partials_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, st>>>(part, out, n, S, stride);
-  ADN_CHECK_LAUNCH("reduce_partials");
-  return ADN_OK;
-}
-
-int colsum(const float* dz, float* db, int64_t rows, int64_t N, float* part, cudaStream_t st) {
-  const int rps = colsum_slice_rows(rows);
-  const int S2 = (int)ceil_div(rows, rps);
-  dim3 grid((unsigned)ceil_div(N, 32), (unsigned)S2);
-  colsum_partial_kernel<<<grid, 256, 0, st>>>(dz, part, (int)rows, (int)N, rps);
-  ADN_CHECK_LAUNCH("colsum");
-  return reduce_partials(part, db, N, S2, N, st);
-}
-
-// ---- grouped variants: one launch for the same reduction of several subnetworks (blockIdx.z = job) ----
+// ---- one launch for the same reduction of several jobs (blockIdx.z = job) ----
 static constexpr int kMaxJobs = 16;
 struct ReduceJobs { ReduceJob j[kMaxJobs]; };
 struct ColsumJobs { ColsumJob j[kMaxJobs]; int rps[kMaxJobs]; };
@@ -206,12 +161,13 @@ int dense_bwd(const float* x, const float* w, const float* dz, float* dx, float*
     g.C = (S == 1) ? dw : wsf;
     int rc = launch_gemm<true, false, EPI_PARTIAL>(g, S, st, "simt dense_bwd dW");
     if (rc) return rc;
-    if (S > 1 && (rc = reduce_partials(wsf, dw, in * out, S, in * out, st))) return rc;
+    const ReduceJob red{wsf, dw, in * out, S, in * out};
+    if (S > 1 && (rc = reduce_partials_group(&red, 1, st))) return rc;
   }
   // ---- db = colsum(dz) ----
   if (db) {
-    float* part = wsf + (size_t)max_splits(batch) * in * out;
-    int rc = colsum(dz, db, batch, out, part, st);
+    const ColsumJob job{dz, db, batch, out, wsf + (size_t)max_splits(batch) * in * out};
+    int rc = colsum_group(&job, 1, st);
     if (rc) return rc;
   }
   // ---- dx = (dz @ w^T) * relu_mask(x) ----

@@ -141,16 +141,13 @@ sgemm_kernel(GemmArgs g) {
   }
 }
 
-// out[i] = sum_{s<S} part[s*stride + i]   (fixed order -> deterministic)
-int reduce_partials(const float* part, float* out, int64_t n, int S, int64_t stride, cudaStream_t st);
-// grouped: out[i] = sum_s part[s*stride + i] for several (part, out) pairs in one launch
+// out[i] = scale * sum_{s<S} part[s*stride + i] (fixed order -> deterministic) for several jobs in one launch
 struct ReduceJob { const float* part; float* out; int64_t n; int S; int64_t stride; float scale = 1.0f; };   // out = scale * sum
 int reduce_partials_group(const ReduceJob* jobs, int n, cudaStream_t st);
-// grouped column sums: out[c] = sum_r x[r, c]; part = 64 * cols floats of scratch per job
+// column sums out[c] = scale * sum_r x[r, c] via fixed-order partials for several jobs in one launch (+ one reduce
+// launch); part = 64 * cols floats of scratch per job
 struct ColsumJob { const float* x; float* out; int64_t rows, cols; float* part; float scale = 1.0f; };
 int colsum_group(const ColsumJob* jobs, int n, cudaStream_t st);
-// db[n] = sum_rows dz[row*N + n] via fixed-order partials in `part` (ceil(rows/512)*N floats)
-int colsum(const float* dz, float* db, int64_t rows, int64_t N, float* part, cudaStream_t st);
 
 int dense_fwd(const float* x, const float* w, const float* b, float* y, int64_t batch, int64_t in,
               int64_t out, int act, cudaStream_t st);

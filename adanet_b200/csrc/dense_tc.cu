@@ -83,7 +83,8 @@ int dense_bwd(const float* x, const float* w, const float* dz, float* dx, float*
   if ((rc = pl::split(pl::FMT_TF32, x, batch, in, xp, 0, st))) return rc;     // also yields the sign bits used as the ReLU mask
   if ((rc = pl::split(pl::FMT_TF32, dz, batch, out, dzp, 0, st))) return rc;
   if (dx && (rc = pl::split(pl::FMT_TF32, w, in, out, wp, 0, st))) return rc;
-  if (db && (rc = simt::colsum(dz, db, batch, out, dbpart, st))) return rc;
+  const simt::ColsumJob db_job{dz, db, batch, out, dbpart};
+  if (db && (rc = simt::colsum_group(&db_job, 1, st))) return rc;
   return pl::dense_bwd(pl::FMT_TF32, xp, wp, dzp, nullptr, dx, nullptr, dw, batch, in, out, x_relu_mask, 0, inner_ws, inner, st);
 }
 

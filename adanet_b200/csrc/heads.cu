@@ -2,6 +2,9 @@
 // and L1 norm.  HBM-bound: every member-logit element is read from DRAM once
 // (pass 1), re-read from L2 for the mixture-weight gradient (pass 2), with
 // coalesced float4 loads over the flat [rows*dim] tile of each member.
+// Every head entry point (adn_head_group, adn_ensemble_head, adn_head_loss(_p))
+// goes through one validator (head_group_op) and one launcher (run_heads) of one
+// kernel family: a single head is a one-op group.
 //
 // Reference arithmetic being replaced (file:line in tensorflow/adanet v0.9.0):
 //   weighted logits / sum    adanet/ensemble/weighted.py:433-453,545-561
@@ -249,16 +252,9 @@ __device__ __forceinline__ void head_body(const HeadParams& p, float* smem, cons
   }
 }
 
-template <int CT>
-__global__ void __launch_bounds__(kRows)
-ensemble_head_kernel(const __grid_constant__ HeadParams p) {
-  extern __shared__ __align__(16) float smem[];
-  head_body<CT>(p, smem, blockIdx.x);
-}
-
-// Grouped form: blockIdx.y selects one of up to kMaxGroup independent heads over the same minibatch -- the
-// subnetwork losses and the candidate-ensemble heads of every candidate of the GPU in ONE launch (they only read
-// logits the forward waves have produced), instead of two launches per candidate on side streams.
+// blockIdx.y selects one of up to kMaxGroup independent heads over the same minibatch -- the subnetwork losses and
+// the candidate-ensemble heads of every candidate of the GPU in ONE launch (they only read logits the forward waves
+// have produced), instead of two launches per candidate on side streams.
 static constexpr int kMaxGroup = 24;
 struct HeadGroup {
   HeadParams p[kMaxGroup];
@@ -348,10 +344,6 @@ __device__ __forceinline__ void finalize_body(const HeadParams& p, const float* 
 }
 
 __global__ void __launch_bounds__(256)
-ensemble_finalize_kernel(const __grid_constant__ HeadParams p, const float* __restrict__ part, int n_cta) {
-  finalize_body(p, part, n_cta);
-}
-__global__ void __launch_bounds__(256)
 ensemble_finalize_group_kernel(const __grid_constant__ HeadGroup g) {
   const HeadParams& p = g.p[blockIdx.x];
   finalize_body(p, p.part, p.n_cta);
@@ -422,51 +414,22 @@ static size_t head_smem_bytes(int dim, int members) {
   return ((size_t)(members + 1) * kRows * dim + (size_t)(kRows / 32) * wr) * sizeof(float);
 }
 
-static int run_head(HeadParams& p, void* ws, int64_t ws_bytes, cudaStream_t st) {
-  if (p.batch <= 0 || p.dim <= 0) return fail(ADN_ERR_INVALID, "head: empty batch/dim");
-  if (p.dim > kMaxDim) return fail(ADN_ERR_UNSUPPORTED, "head: dim %d > %d", p.dim, kMaxDim);
-  if (p.n_members < 1 || p.n_members > kMaxMembers)
-    return fail(ADN_ERR_UNSUPPORTED, "head: n_members %d not in [1,%d]", p.n_members, kMaxMembers);
-  if (p.head == ADN_HEAD_SOFTMAX_XENT ? p.labels == nullptr : p.labels_f == nullptr)
-    return fail(ADN_ERR_INVALID, "head: labels missing for head kind %d", p.head);
-  const int wdim = (p.mixture == ADN_MIX_SCALAR) ? 1 : p.dim;
-  p.n_out = 1 + p.dim + p.n_members * wdim;
-  if (ws_bytes < head_workspace_bytes(p.batch, p.dim, p.n_members))
-    return fail(ADN_ERR_WORKSPACE, "head: workspace %lld < %lld bytes", (long long)ws_bytes,
-                (long long)head_workspace_bytes(p.batch, p.dim, p.n_members));
-  p.part = reinterpret_cast<float*>(ws);
-  const int n_cta = (int)ceil_div(p.batch, kRows);
-  p.n_cta = n_cta;
-  const size_t smem = head_smem_bytes(p.dim, p.n_members);
-  if (smem > 227 * 1024)
-    return fail(ADN_ERR_UNSUPPORTED, "head: n_members*dim = %d*%d does not fit shared memory", p.n_members, p.dim);
-  switch (p.dim) {
-    case 1: ensemble_head_kernel<1><<<n_cta, kRows, smem, st>>>(p); break;
-    case 2: ensemble_head_kernel<2><<<n_cta, kRows, smem, st>>>(p); break;
-    case 3: ensemble_head_kernel<3><<<n_cta, kRows, smem, st>>>(p); break;
-    case 4: ensemble_head_kernel<4><<<n_cta, kRows, smem, st>>>(p); break;
-    case 10: ensemble_head_kernel<10><<<n_cta, kRows, smem, st>>>(p); break;
-    case 16: ensemble_head_kernel<16><<<n_cta, kRows, smem, st>>>(p); break;
-    default: ensemble_head_kernel<0><<<n_cta, kRows, smem, st>>>(p); break;
+static void launch_head_group(const HeadGroup& g, int n_cta, size_t smem, cudaStream_t st) {
+  const dim3 grid((unsigned)n_cta, (unsigned)g.n);
+  switch (g.p[0].dim) {    // every op of a call shares dim
+    case 1: ensemble_head_group_kernel<1><<<grid, kRows, smem, st>>>(g); break;
+    case 2: ensemble_head_group_kernel<2><<<grid, kRows, smem, st>>>(g); break;
+    case 3: ensemble_head_group_kernel<3><<<grid, kRows, smem, st>>>(g); break;
+    case 4: ensemble_head_group_kernel<4><<<grid, kRows, smem, st>>>(g); break;
+    case 10: ensemble_head_group_kernel<10><<<grid, kRows, smem, st>>>(g); break;
+    case 16: ensemble_head_group_kernel<16><<<grid, kRows, smem, st>>>(g); break;
+    default: ensemble_head_group_kernel<0><<<grid, kRows, smem, st>>>(g); break;
   }
-  ADN_CHECK_LAUNCH("ensemble_head");
-  if (n_cta > 512) {
-    // many CTAs (large batches): one block per output sums its partials first, the finalize then sees one row
-    const int n_red = p.want_grads ? (1 + p.dim + ((p.mixture == ADN_MIX_MATRIX || p.colsum_only) ? 0 : p.n_members * wdim)) : 1;
-    float* red = p.part + (size_t)n_cta * p.n_out;
-    head_partials_kernel<<<n_red, 256, 0, st>>>(p.part, red, n_cta);
-    ADN_CHECK_LAUNCH("head_partials");
-    ensemble_finalize_kernel<<<1, 256, 0, st>>>(p, red, 1);
-  } else {
-    ensemble_finalize_kernel<<<1, 256, 0, st>>>(p, p.part, n_cta);
-  }
-  ADN_CHECK_LAUNCH("ensemble_finalize");
-  return ADN_OK;
 }
 
 int heads_init() {
 #define ADN_HEAD_ATTR(CT) \
-  ADN_CUDA(cudaFuncSetAttribute(ensemble_head_kernel<CT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024))
+  ADN_CUDA(cudaFuncSetAttribute(ensemble_head_group_kernel<CT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024))
   ADN_HEAD_ATTR(0); ADN_HEAD_ATTR(1); ADN_HEAD_ATTR(2); ADN_HEAD_ATTR(3); ADN_HEAD_ATTR(4); ADN_HEAD_ATTR(10);
   ADN_HEAD_ATTR(16);
 #undef ADN_HEAD_ATTR
@@ -477,146 +440,21 @@ int64_t head_workspace_bytes_public(int64_t batch, int64_t dim, int64_t members)
   return head_workspace_bytes(batch, dim, members < 1 ? 1 : members);
 }
 
-}  // namespace adn
-
-using namespace adn;
-
-
-extern "C" int adn_head_loss(int head, const float* logits, const int64_t* labels, const float* labels_f,
-                             float* loss_out, float* dlogits, int64_t batch, int64_t dim,
-                             void* workspace, int64_t workspace_bytes, void* stream) {
-  return adn_head_loss_p(head, logits, labels, labels_f, loss_out, dlogits, nullptr, nullptr, 0, batch, dim, workspace,
-                         workspace_bytes, stream);
-}
-
-extern "C" int adn_head_loss_p(int head, const float* logits, const int64_t* labels, const float* labels_f,
-                               float* loss_out, float* dlogits, void* dlogits_planes, float* dlogits_colsum,
-                               int dz_log2_scale, int64_t batch, int64_t dim, void* workspace, int64_t workspace_bytes,
-                               void* stream) {
-  if (!logits || !loss_out) return fail(ADN_ERR_INVALID, "adn_head_loss: null pointer");
-  if (head < 0 || head > 2) return fail(ADN_ERR_INVALID, "adn_head_loss: bad head %d", head);
-  // out3 needs 3 floats; the public contract is loss_out[0], so stage through workspace tail.
-  HeadParams p{};
-  p.members[0] = logits;
-  p.n_members = 1;
-  p.head = head;
-  p.mixture = ADN_MIX_SCALAR;
-  p.labels = labels;
-  p.labels_f = labels_f;
-  p.dens = dlogits;
-  if (dz_log2_scale < -60 || dz_log2_scale > 60) return fail(ADN_ERR_INVALID, "adn_head_loss_p: bad dz_log2_scale");
-  if (dlogits_planes) {
-    const int fmt = pl::format();
-    p.densp = pl::plane_view(fmt, dlogits_planes, batch, dim);
-    p.dens_scale = ldexpf(1.0f, dz_log2_scale);
-    p.dens_nkb = (int)ceil_div(dim, pl::fmt_bk(fmt));
-    p.ovf = pl::overflow_flag();
-  }
-  p.batch = batch;
-  p.dim = (int)dim;
-  p.want_grads = dlogits_colsum ? 1 : 0;
-  p.colsum_only = 1;
-  p.dbias = dlogits_colsum;
-  p.reg_is_zero = 1;
-  const int64_t need = head_workspace_bytes_public(batch, dim, 1);
-  if (workspace_bytes < need + 16)
-    return fail(ADN_ERR_WORKSPACE, "adn_head_loss: workspace %lld < %lld bytes", (long long)workspace_bytes,
-                (long long)(need + 16));
-  float* out3 = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + need);
-  p.out3 = out3;
-  int rc = run_head(p, workspace, need, as_stream(stream));
-  if (rc) return rc;
-  ADN_CUDA(cudaMemcpyAsync(loss_out, out3, sizeof(float), cudaMemcpyDeviceToDevice, as_stream(stream)));
-  return ADN_OK;
-}
-
-extern "C" int adn_ensemble_head(int head, int mixture_type, const float* const* members_host, int n_members,
-                                 const float* w, const float* bias, const float* gammas_host, int reg_is_zero,
-                                 float reg_multiplier, const int64_t* labels, const float* labels_f,
-                                 float* out3, float* dw, float* dbias, float* dens, float* ens_out,
-                                 int64_t batch, int64_t dim, void* workspace, int64_t workspace_bytes,
-                                 void* stream) {
-  if (!members_host || !out3) return fail(ADN_ERR_INVALID, "adn_ensemble_head: null pointer");
-  if (head < 0 || head > 2) return fail(ADN_ERR_INVALID, "adn_ensemble_head: bad head %d", head);
-  if (mixture_type < 0 || mixture_type > 2)
-    return fail(ADN_ERR_INVALID, "adn_ensemble_head: bad mixture type %d", mixture_type);
-  if (n_members < 1 || n_members > kMaxMembers)
-    return fail(ADN_ERR_UNSUPPORTED, "adn_ensemble_head: n_members %d not in [1,%d]", n_members, kMaxMembers);
-  if (mixture_type == ADN_MIX_MATRIX && dw)
-    return fail(ADN_ERR_INVALID, "adn_ensemble_head: dw must be NULL for MATRIX mixture weights");
-  if (!reg_is_zero && !gammas_host) return fail(ADN_ERR_INVALID, "adn_ensemble_head: gammas missing");
-  HeadParams p{};
-  for (int k = 0; k < n_members; ++k) {
-    if (!members_host[k]) return fail(ADN_ERR_INVALID, "adn_ensemble_head: member %d is null", k);
-    p.members[k] = members_host[k];
-    p.gammas[k] = gammas_host ? gammas_host[k] : 0.f;
-  }
-  p.n_members = n_members;
-  p.head = head;
-  p.mixture = mixture_type;
-  p.w = w;
-  p.bias = bias;
-  p.labels = labels;
-  p.labels_f = labels_f;
-  p.dens = dens;
-  p.ens_out = ens_out;
-  p.batch = batch;
-  p.dim = (int)dim;
-  p.want_grads = (dw || dbias) ? 1 : 0;
-  p.reg_is_zero = reg_is_zero;
-  p.reg_multiplier = reg_multiplier;
-  p.out3 = out3;
-  p.dw = dw;
-  p.dbias = dbias;
-  return run_head(p, workspace, workspace_bytes, as_stream(stream));
-}
-
-extern "C" int adn_ema_update(float* state, const float* loss, float decay, void* stream) {
-  if (!state || !loss) return fail(ADN_ERR_INVALID, "adn_ema_update: null pointer");
-  ema_update_kernel<<<1, 1, 0, as_stream(stream)>>>(state, loss, decay);
-  ADN_CHECK_LAUNCH("ema_update");
-  return ADN_OK;
-}
-
-extern "C" int adn_l1_norm(const float* x, int64_t n, float* out, void* stream) {
-  if (!x || !out || n < 0) return fail(ADN_ERR_INVALID, "adn_l1_norm: bad argument");
-  l1_norm_kernel<<<1, 1024, 0, as_stream(stream)>>>(x, n, out);
-  ADN_CHECK_LAUNCH("l1_norm");
-  return ADN_OK;
-}
-
-
-// ---- grouped heads (include/adanet_b200.h: adn_head_group / adn_head_bookkeeping) ----
-namespace adn {
-template <int CT>
-static void launch_head_group(const HeadGroup& g, int n_cta, size_t smem, cudaStream_t st) {
-  ensemble_head_group_kernel<CT><<<dim3((unsigned)n_cta, (unsigned)g.n), kRows, smem, st>>>(g);
-}
-int heads_group_init() {
-#define ADN_HEADG_ATTR(CT) \
-  ADN_CUDA(cudaFuncSetAttribute(ensemble_head_group_kernel<CT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024))
-  ADN_HEADG_ATTR(0); ADN_HEADG_ATTR(1); ADN_HEADG_ATTR(2); ADN_HEADG_ATTR(3); ADN_HEADG_ATTR(4); ADN_HEADG_ATTR(10);
-  ADN_HEADG_ATTR(16);
-#undef ADN_HEADG_ATTR
-  return ADN_OK;
-}
-}  // namespace adn
-
-namespace adn {
-// Checks op `idx` of adn_head_group and fills its launch parameters; touches no device memory.
-static int head_group_op(const adn_head_op& o, int idx, int64_t batch, int64_t dim, int fmt, int n_cta, HeadParams& p) {
-  if (!o.members_host || !o.out3 || !o.workspace) return fail(ADN_ERR_INVALID, "adn_head_group: op %d: null pointer", idx);
+// Checks one op (`what` names it in messages) and fills its launch parameters; touches no device memory.
+static int head_group_op(const adn_head_op& o, const char* what, int64_t batch, int64_t dim, int fmt, int n_cta,
+                         HeadParams& p) {
+  if (!o.members_host || !o.out3 || !o.workspace) return fail(ADN_ERR_INVALID, "%s: null pointer", what);
   if (o.head < 0 || o.head > 2 || o.mixture_type < 0 || o.mixture_type > 2)
-    return fail(ADN_ERR_INVALID, "adn_head_group: op %d: bad head / mixture type", idx);
+    return fail(ADN_ERR_INVALID, "%s: bad head / mixture type (%d, %d)", what, o.head, o.mixture_type);
   if (o.n_members < 1 || o.n_members > kMaxMembers)
-    return fail(ADN_ERR_UNSUPPORTED, "adn_head_group: op %d: n_members %d not in [1,%d]", idx, o.n_members, kMaxMembers);
-  if (o.mixture_type == ADN_MIX_MATRIX && o.dw) return fail(ADN_ERR_INVALID, "adn_head_group: op %d: dw must be NULL for MATRIX", idx);
-  if (!o.reg_is_zero && !o.gammas_host) return fail(ADN_ERR_INVALID, "adn_head_group: op %d: gammas missing", idx);
+    return fail(ADN_ERR_UNSUPPORTED, "%s: n_members %d not in [1,%d]", what, o.n_members, kMaxMembers);
+  if (o.mixture_type == ADN_MIX_MATRIX && o.dw) return fail(ADN_ERR_INVALID, "%s: dw must be NULL for MATRIX", what);
+  if (!o.reg_is_zero && !o.gammas_host) return fail(ADN_ERR_INVALID, "%s: gammas missing", what);
   if (o.head == ADN_HEAD_SOFTMAX_XENT ? o.labels == nullptr : o.labels_f == nullptr)
-    return fail(ADN_ERR_INVALID, "adn_head_group: op %d: labels missing", idx);
-  if (o.dz_log2_scale < -60 || o.dz_log2_scale > 60) return fail(ADN_ERR_INVALID, "adn_head_group: op %d: bad dz_log2_scale", idx);
+    return fail(ADN_ERR_INVALID, "%s: labels missing", what);
+  if (o.dz_log2_scale < -60 || o.dz_log2_scale > 60) return fail(ADN_ERR_INVALID, "%s: bad dz_log2_scale", what);
   for (int k = 0; k < o.n_members; ++k) {
-    if (!o.members_host[k]) return fail(ADN_ERR_INVALID, "adn_head_group: op %d: member %d is null", idx, k);
+    if (!o.members_host[k]) return fail(ADN_ERR_INVALID, "%s: member %d is null", what, k);
     p.members[k] = o.members_host[k];
     p.gammas[k] = o.gammas_host ? o.gammas_host[k] : 0.f;
   }
@@ -647,67 +485,169 @@ static int head_group_op(const adn_head_op& o, int idx, int64_t batch, int64_t d
   const int wdim = (p.mixture == ADN_MIX_SCALAR) ? 1 : p.dim;
   p.n_out = 1 + p.dim + p.n_members * wdim;
   if (o.workspace_bytes < head_workspace_bytes(batch, dim, o.n_members))
-    return fail(ADN_ERR_WORKSPACE, "adn_head_group: op %d: workspace %lld < %lld bytes", idx, (long long)o.workspace_bytes,
+    return fail(ADN_ERR_WORKSPACE, "%s: workspace %lld < %lld bytes", what, (long long)o.workspace_bytes,
                 (long long)head_workspace_bytes(batch, dim, o.n_members));
   p.part = reinterpret_cast<float*>(o.workspace);
   p.n_cta = n_cta;
   return ADN_OK;
 }
 
-// Fills the launch of ops [i0, i0 + g.n) and the shared memory it needs.
+// Fills the launch of ops [i0, i0 + m) and the shared memory it needs.  A grouped call (`per_op`) names each op by
+// its index after `what`.
 static int head_group_chunk(const adn_head_op* ops, int i0, int m, int64_t batch, int64_t dim, int fmt, int n_cta,
-                            HeadGroup& g, size_t& smem) {
+                            const char* what, bool per_op, HeadGroup& g, size_t& smem) {
   g = HeadGroup{};
   g.n = m;
   smem = 0;
   for (int i = 0; i < m; ++i) {
-    const int rc = head_group_op(ops[i0 + i], i0 + i, batch, dim, fmt, n_cta, g.p[i]);
+    char name[64];
+    if (per_op) snprintf(name, sizeof(name), "%s: op %d", what, i0 + i);
+    const int rc = head_group_op(ops[i0 + i], per_op ? name : what, batch, dim, fmt, n_cta, g.p[i]);
     if (rc) return rc;
     smem = std::max(smem, head_smem_bytes(g.p[i].dim, g.p[i].n_members));
   }
-  if (smem > 227 * 1024) return fail(ADN_ERR_UNSUPPORTED, "adn_head_group: members x dim does not fit shared memory");
+  if (smem > 227 * 1024) return fail(ADN_ERR_UNSUPPORTED, "%s: members x dim does not fit shared memory", what);
   return ADN_OK;
 }
-}  // namespace adn
 
-extern "C" int adn_head_group(const adn_head_op* ops, int n, int64_t batch, int64_t dim, void* stream) {
-  if (n < 0 || (n > 0 && !ops)) return fail(ADN_ERR_INVALID, "adn_head_group: bad ops");
-  if (batch <= 0 || dim <= 0 || dim > kMaxDim) return fail(ADN_ERR_INVALID, "adn_head_group: bad batch/dim");
+// Every head entry point: ops over one minibatch, all checked before the first launch, so a rejected call writes
+// nothing.  Up to 512 CTAs per op: one head launch and one finalize launch per kMaxGroup ops.  Beyond (very large
+// batches), op by op: its head launch, one block per output summing the CTA partials of that output, and a finalize
+// that sees the reduced row alone.
+static int run_heads(const adn_head_op* ops, int n, int64_t batch, int64_t dim, const char* what, bool per_op,
+                     cudaStream_t st) {
+  if (batch <= 0 || dim <= 0 || dim > kMaxDim) return fail(ADN_ERR_INVALID, "%s: bad batch/dim", what);
   const int n_cta = (int)ceil_div(batch, kRows);
   const int fmt = pl::format();
-  const bool single_path = n_cta > 512;      // very large batches: two-level finalize of the single-head path
   HeadGroup g;
   size_t smem;
   int rc;
-  // every op is checked before the first launch, so a rejected call writes nothing
   for (int i0 = 0; i0 < n; i0 += kMaxGroup)
-    if ((rc = head_group_chunk(ops, i0, std::min(kMaxGroup, n - i0), batch, dim, fmt, n_cta, g, smem))) return rc;
+    if ((rc = head_group_chunk(ops, i0, std::min(kMaxGroup, n - i0), batch, dim, fmt, n_cta, what, per_op, g, smem)))
+      return rc;
   for (int i0 = 0; i0 < n; i0 += kMaxGroup) {
     const int m = std::min(kMaxGroup, n - i0);
-    if ((rc = head_group_chunk(ops, i0, m, batch, dim, fmt, n_cta, g, smem))) return rc;
-    if (single_path) {
-      for (int i = 0; i < m; ++i) {
-        const adn_head_op& o = ops[i0 + i];
-        if ((rc = run_head(g.p[i], o.workspace, o.workspace_bytes, as_stream(stream)))) return rc;
-      }
+    if ((rc = head_group_chunk(ops, i0, m, batch, dim, fmt, n_cta, what, per_op, g, smem))) return rc;
+    if (n_cta <= 512) {
+      launch_head_group(g, n_cta, smem, st);
+      ADN_CHECK_LAUNCH("ensemble_head_group");
+      ensemble_finalize_group_kernel<<<m, 256, 0, st>>>(g);
+      ADN_CHECK_LAUNCH("ensemble_finalize_group");
       continue;
     }
-    cudaStream_t st = as_stream(stream);
-    switch ((int)dim) {
-      case 1: launch_head_group<1>(g, n_cta, smem, st); break;
-      case 2: launch_head_group<2>(g, n_cta, smem, st); break;
-      case 3: launch_head_group<3>(g, n_cta, smem, st); break;
-      case 4: launch_head_group<4>(g, n_cta, smem, st); break;
-      case 10: launch_head_group<10>(g, n_cta, smem, st); break;
-      case 16: launch_head_group<16>(g, n_cta, smem, st); break;
-      default: launch_head_group<0>(g, n_cta, smem, st); break;
+    for (int i = 0; i < m; ++i) {
+      HeadGroup one{};
+      one.n = 1;
+      HeadParams& p = one.p[0];
+      p = g.p[i];
+      launch_head_group(one, n_cta, head_smem_bytes(p.dim, p.n_members), st);
+      ADN_CHECK_LAUNCH("ensemble_head_group");
+      const int n_red = !p.want_grads ? 1 : (p.mixture == ADN_MIX_MATRIX || p.colsum_only) ? 1 + p.dim : p.n_out;
+      float* red = p.part + (size_t)n_cta * p.n_out;
+      head_partials_kernel<<<n_red, 256, 0, st>>>(p.part, red, n_cta);
+      ADN_CHECK_LAUNCH("head_partials");
+      p.part = red;
+      p.n_cta = 1;
+      ensemble_finalize_group_kernel<<<1, 256, 0, st>>>(one);
+      ADN_CHECK_LAUNCH("ensemble_finalize_group");
     }
-    ADN_CHECK_LAUNCH("ensemble_head_group");
-    ensemble_finalize_group_kernel<<<m, 256, 0, st>>>(g);
-    ADN_CHECK_LAUNCH("ensemble_finalize_group");
   }
   return ADN_OK;
 }
+
+}  // namespace adn
+
+using namespace adn;
+
+extern "C" int adn_head_loss(int head, const float* logits, const int64_t* labels, const float* labels_f,
+                             float* loss_out, float* dlogits, int64_t batch, int64_t dim,
+                             void* workspace, int64_t workspace_bytes, void* stream) {
+  return adn_head_loss_p(head, logits, labels, labels_f, loss_out, dlogits, nullptr, nullptr, 0, batch, dim, workspace,
+                         workspace_bytes, stream);
+}
+
+extern "C" int adn_head_loss_p(int head, const float* logits, const int64_t* labels, const float* labels_f,
+                               float* loss_out, float* dlogits, void* dlogits_planes, float* dlogits_colsum,
+                               int dz_log2_scale, int64_t batch, int64_t dim, void* workspace, int64_t workspace_bytes,
+                               void* stream) {
+  if (!logits || !loss_out) return fail(ADN_ERR_INVALID, "adn_head_loss_p: null pointer");
+  // out3 needs 3 floats; the public contract is loss_out[0], so stage through workspace tail.
+  const int64_t need = head_workspace_bytes_public(batch, dim, 1);
+  if (workspace_bytes < need + 16)
+    return fail(ADN_ERR_WORKSPACE, "adn_head_loss_p: workspace %lld < %lld bytes", (long long)workspace_bytes,
+                (long long)(need + 16));
+  if (dim > kMaxDim) return fail(ADN_ERR_UNSUPPORTED, "adn_head_loss_p: dim %lld > %d", (long long)dim, kMaxDim);
+  float* out3 = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + need);
+  adn_head_op o{};
+  o.head = head;
+  o.mixture_type = ADN_MIX_SCALAR;
+  o.members_host = &logits;
+  o.n_members = 1;
+  o.reg_is_zero = 1;
+  o.dz_log2_scale = dz_log2_scale;
+  o.labels = labels;
+  o.labels_f = labels_f;
+  o.out3 = out3;
+  o.dbias = dlogits_colsum;
+  o.dens = dlogits;
+  o.dens_planes = dlogits_planes;
+  o.colsum_only = 1;
+  o.workspace = workspace;
+  o.workspace_bytes = need;
+  const int rc = run_heads(&o, 1, batch, dim, "adn_head_loss_p", false, as_stream(stream));
+  if (rc) return rc;
+  ADN_CUDA(cudaMemcpyAsync(loss_out, out3, sizeof(float), cudaMemcpyDeviceToDevice, as_stream(stream)));
+  return ADN_OK;
+}
+
+extern "C" int adn_ensemble_head(int head, int mixture_type, const float* const* members_host, int n_members,
+                                 const float* w, const float* bias, const float* gammas_host, int reg_is_zero,
+                                 float reg_multiplier, const int64_t* labels, const float* labels_f,
+                                 float* out3, float* dw, float* dbias, float* dens, float* ens_out,
+                                 int64_t batch, int64_t dim, void* workspace, int64_t workspace_bytes,
+                                 void* stream) {
+  if (dim > kMaxDim) return fail(ADN_ERR_UNSUPPORTED, "adn_ensemble_head: dim %lld > %d", (long long)dim, kMaxDim);
+  adn_head_op o{};
+  o.head = head;
+  o.mixture_type = mixture_type;
+  o.members_host = members_host;
+  o.n_members = n_members;
+  o.reg_is_zero = reg_is_zero;
+  o.w = w;
+  o.bias = bias;
+  o.gammas_host = gammas_host;
+  o.reg_multiplier = reg_multiplier;
+  o.labels = labels;
+  o.labels_f = labels_f;
+  o.out3 = out3;
+  o.dw = dw;
+  o.dbias = dbias;
+  o.dens = dens;
+  o.ens_out = ens_out;
+  o.workspace = workspace;
+  o.workspace_bytes = workspace_bytes;
+  return run_heads(&o, 1, batch, dim, "adn_ensemble_head", false, as_stream(stream));
+}
+
+extern "C" int adn_head_group(const adn_head_op* ops, int n, int64_t batch, int64_t dim, void* stream) {
+  if (n < 0 || (n > 0 && !ops)) return fail(ADN_ERR_INVALID, "adn_head_group: bad ops");
+  return run_heads(ops, n, batch, dim, "adn_head_group", true, as_stream(stream));
+}
+
+extern "C" int adn_ema_update(float* state, const float* loss, float decay, void* stream) {
+  if (!state || !loss) return fail(ADN_ERR_INVALID, "adn_ema_update: null pointer");
+  ema_update_kernel<<<1, 1, 0, as_stream(stream)>>>(state, loss, decay);
+  ADN_CHECK_LAUNCH("ema_update");
+  return ADN_OK;
+}
+
+extern "C" int adn_l1_norm(const float* x, int64_t n, float* out, void* stream) {
+  if (!x || !out || n < 0) return fail(ADN_ERR_INVALID, "adn_l1_norm: bad argument");
+  l1_norm_kernel<<<1, 1024, 0, as_stream(stream)>>>(x, n, out);
+  ADN_CHECK_LAUNCH("l1_norm");
+  return ADN_OK;
+}
+
 
 extern "C" int adn_head_bookkeeping(const adn_head_book* books, int n, const int64_t* step_dev, void* stream) {
   if (n < 0 || (n > 0 && !books) || !step_dev) return fail(ADN_ERR_INVALID, "adn_head_bookkeeping: bad argument");

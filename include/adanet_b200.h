@@ -139,6 +139,7 @@ int adn_dense_bwd(const float* x, const float* w, const float* dz,
  * Replaces head.create_estimator_spec(...).loss on subnetwork logits,
  *   adanet/core/ensemble_builder.py:756-758 (+ :571-583).
  * workspace: adn_query(ADN_Q_HEAD_WORKSPACE_BYTES, batch, dim, 1).
+ * = adn_head_loss_p(..., dlogits_planes = NULL, dlogits_colsum = NULL, dz_log2_scale = 0, ...).
  */
 int adn_head_loss(int head, const float* logits, const int64_t* labels, const float* labels_f,
                   float* loss_out, float* dlogits, int64_t batch, int64_t dim,
@@ -163,6 +164,8 @@ int adn_head_loss(int head, const float* logits, const int64_t* labels, const fl
  * dw (nullable): same shape as w.  dbias (nullable): [dim].
  * dens (nullable): [batch,dim] dLoss/d(ens) (needed for MATRIX weight grads).
  * ens_out (nullable): [batch,dim] ensemble logits (predict / evaluate).
+ * A one-op adn_head_group: the adn_head_op of the same fields, colsum_only = 0, dz_log2_scale = 0, dens_planes =
+ * NULL; errors as there, except dim > 64 is ADN_ERR_UNSUPPORTED.
  */
 int adn_ensemble_head(int head, int mixture_type, const float* const* members_host, int n_members,
                       const float* w, const float* bias, const float* gammas_host, int reg_is_zero,
@@ -209,14 +212,15 @@ int adn_planes_split(const float* src, int64_t rows, int64_t cols, void* planes,
 int adn_planes_split_scaled(const float* src, int64_t rows, int64_t cols, void* planes, int log2_scale, void* stream);
 int adn_planes_merge(const void* planes, int64_t rows, int64_t cols, float* dst, void* stream);
 /* y = act(x @ w + b): xp planes [batch,in], wp planes [in,out]; result as planes (yp) or
- * dense fp32 row-major (y) -- exactly one of the two is non-NULL. */
+ * dense fp32 row-major (y) -- exactly one of the two is non-NULL.  A one-op adn_dense_fwd_p_group: bias = b, no
+ * dropout, n_srcs = 0. */
 int adn_dense_fwd_p(const void* xp, const void* wp, const float* b, void* yp, float* y,
                     int64_t batch, int64_t in, int64_t out, int act, void* stream);
 /* Backward of one dense layer from planes: dzp planes [batch,out] holding dz * 2^dz_log2_scale.
  *   dw[in,out] (dense, nullable) = x^T dz
  *   dx = (dz w^T) * (x_relu_mask ? x > 0 : 1) as planes (dxp) or dense (dx); both may be NULL
  *   dx_colsum[in] (nullable) = column sums of dx = the bias gradient of the layer below
- * workspace: adn_query(ADN_Q_DENSE_BWD_P_WORKSPACE_BYTES). */
+ * workspace: adn_query(ADN_Q_DENSE_BWD_P_WORKSPACE_BYTES).  A one-op adn_dense_bwd_p_group: dx_mul = 1. */
 int adn_dense_bwd_p(const void* xp, const void* wp, const void* dzp, void* dxp, float* dx,
                     float* dx_colsum, float* dw, int64_t batch, int64_t in, int64_t out,
                     int x_relu_mask, int dz_log2_scale, void* workspace, int64_t workspace_bytes, void* stream);
@@ -224,7 +228,7 @@ int adn_dense_bwd_p(const void* xp, const void* wp, const void* dzp, void* dxp, 
  * Grouped forms: the same layer wave of several subnetworks (all candidates of an AdaNet iteration consume
  * the same minibatch, adanet/core/iteration.py:185-192) in ONE persistent launch per GEMM kind, so launch,
  * prologue and pipeline fill/drain are paid once per wave and narrow candidates hide behind wide ones.
- * Per-op semantics are exactly adn_dense_fwd_p / adn_dense_bwd_p; ops must not alias each other's outputs.
+ * Each op is checked before anything is launched; ops must not alias each other's outputs.
  */
 /* One more input piece of a multi-source forward op: planes xp [batch, in] and the matching rows of the layer's
  * kernel as their own planes wp [in, out].  A dense layer over concat([x_0, x_1, ...], axis=-1) with kernel
@@ -286,7 +290,11 @@ int adn_dense_bwd_p_group(const adn_bwd_op* ops_host, int n, int64_t batch, void
 
 /* adn_head_loss that also emits, in the same pass, dlogits * 2^dz_log2_scale as split planes (nullable) and the
  * (un-scaled) column sums of dlogits = the bias gradient of the logits layer (nullable): what the backward
- * GEMMs consume. */
+ * GEMMs consume.  A one-op adn_head_group: head, members_host = &logits, n_members = 1, mixture_type = SCALAR,
+ * reg_is_zero = 1, colsum_only = 1, labels, labels_f, dens = dlogits, dens_planes = dlogits_planes, dz_log2_scale,
+ * dbias = dlogits_colsum, out3 = 16 bytes of the workspace past the op's own share, then loss_out[0] = out3[0].
+ * workspace: adn_query(ADN_Q_HEAD_WORKSPACE_BYTES, batch, dim, 1).  Errors as adn_head_group, except dim > 64 is
+ * ADN_ERR_UNSUPPORTED. */
 int adn_head_loss_p(int head, const float* logits, const int64_t* labels, const float* labels_f,
                     float* loss_out, float* dlogits, void* dlogits_planes, float* dlogits_colsum,
                     int dz_log2_scale, int64_t batch, int64_t dim, void* workspace, int64_t workspace_bytes,
@@ -304,34 +312,39 @@ int adn_opt_step_p(int kind, float* const* params_host, const float* const* grad
 
 /*
  * Grouped heads: every subnetwork loss and every candidate-ensemble head of the candidates on one GPU in ONE launch
- * (plus one finalize launch), over the same minibatch.  Each op is one adn_ensemble_head call (colsum_only = 0) or one
- * adn_head_loss_p call (colsum_only = 1: members_host[0] = the logits, out3[0] = mean loss, dens / dens_planes =
- * dlogits dense / as planes times 2^dz_log2_scale, dbias = column sums of dlogits = the logits-layer bias gradient).
- * All ops share batch and dim.  workspace: adn_query(ADN_Q_HEAD_WORKSPACE_BYTES, batch, dim, n_members), one per op.
- * Every op is checked before anything is launched: a call that returns an error has written nothing.
+ * (plus one finalize launch) per 24 ops, over the same minibatch; above 512 CTAs (batch > 65536) op by op, three
+ * launches each.  adn_ensemble_head and adn_head_loss(_p) are one-op calls of it.  All ops share batch (> 0) and
+ * dim (1..64).  Every op is checked before anything is launched: a call that returns an error has written nothing.
+ * An op is an ensemble head (colsum_only = 0) over n_members member logits:
+ *   out3 = {loss, reg, loss + reg} of ens = bias + sum_k w_k (.) member_k (adn_ensemble_head), and on request
+ *   dw = d(loss + reg_multiplier * reg)/dw, dbias, dens = dLoss/d(ens), ens_out = ens.
+ * or a subnetwork loss (colsum_only = 1): members_host[0] = the logits (n_members = 1), out3[0] = mean loss,
+ * dens / dens_planes = dlogits dense / as planes times 2^dz_log2_scale, dbias = column sums of dlogits = the
+ * logits-layer bias gradient; w, bias, gammas and dw are ignored and reg = 0.
  */
 typedef struct adn_head_op {
   int32_t head;              /* ADN_HEAD_* */
-  int32_t mixture_type;      /* ADN_MIX_* */
-  const float* const* members_host;
-  int32_t n_members;
-  int32_t reg_is_zero;
-  const float* w;
-  const float* bias;
-  const float* gammas_host;
-  float reg_multiplier;
-  int32_t dz_log2_scale;
-  const int64_t* labels;
-  const float* labels_f;
-  float* out3;
-  float* dw;
-  float* dbias;
-  float* dens;
-  float* ens_out;
-  void* dens_planes;
-  int32_t colsum_only;
+  int32_t mixture_type;      /* ADN_MIX_*; SCALAR for a subnetwork loss */
+  const float* const* members_host; /* host array of n_members device pointers to [batch, dim] logits */
+  int32_t n_members;         /* 1..64; members x dim must fit shared memory */
+  int32_t reg_is_zero;       /* 1: lambda == beta == 0, no penalty */
+  const float* w;            /* device: SCALAR [n_members], VECTOR [n_members, dim], MATRIX L1 norms [n_members];
+                                NULL = all 1 */
+  const float* bias;         /* device [dim] or NULL */
+  const float* gammas_host;  /* host [n_members]: lambda * r(h_k) + beta; required unless reg_is_zero */
+  float reg_multiplier;      /* weight of reg in dw (see adn_ensemble_head) */
+  int32_t dz_log2_scale;     /* -60..60: dens_planes hold dLoss/d(ens) * 2^dz_log2_scale */
+  const int64_t* labels;     /* device int64 [batch] class ids (softmax) */
+  const float* labels_f;     /* device [batch, dim] targets (mse / sigmoid) */
+  float* out3;               /* device float[3], required */
+  float* dw;                 /* device, shape of w, or NULL; must be NULL for MATRIX */
+  float* dbias;              /* device [dim] or NULL */
+  float* dens;               /* device [batch, dim] dLoss/d(ens) or NULL */
+  float* ens_out;            /* device [batch, dim] ensemble logits or NULL */
+  void* dens_planes;         /* split planes [batch, dim] of dLoss/d(ens) * 2^dz_log2_scale or NULL */
+  int32_t colsum_only;       /* 1: a subnetwork loss, see above */
   int32_t reserved;
-  void* workspace;
+  void* workspace;           /* device, required: adn_query(ADN_Q_HEAD_WORKSPACE_BYTES, batch, dim, n_members) */
   int64_t workspace_bytes;
 } adn_head_op;
 int adn_head_group(const adn_head_op* ops_host, int n, int64_t batch, int64_t dim, void* stream);

@@ -376,8 +376,9 @@ HEAD_SHAPES = [(1, 1, 9), (127, 2, 9), (128, 3, 9), (129, 4, 9), (1000, 10, 30),
 def test_head_group(env, B, C, n_ops):
   """adn_head_group: every output against float64, the gradient planes byte-identical to adn_planes_split_scaled of
   the kernel's own dlogits (zero padding columns included), the fp16 overflow flag, and every op byte-identical to
-  the same op run alone.  30 and 26 ops take two launches; batch 65537 (> 512 CTAs) runs op by op with the two-level
-  finalize."""
+  the same op run alone (a one-op call of the same launcher), here inside a call of many ops whose launch sizes its
+  shared memory for the largest op.  30 and 26 ops take two launches; batch 65537 (> 512 CTAs) runs op by op, each
+  op as its own one-op head launch, a first-level sum of its CTA partials and a one-op finalize over that row."""
   torch, _lib, lib = env
   f16 = _lib.plane_format() == _lib.PLANES_F16
   inp, rng = _head_inputs(torch, B, C, B * 100 + C)

@@ -92,6 +92,132 @@ def test_cabi_argument_validation_without_gpu(built_lib):
     _lib.check(built_lib.adn_set_dense_path(9), "adn_set_dense_path")
   assert _lib.query(_lib.Q_DENSE_BWD_WS, 4096, 100, 1024) > 0
   assert _lib.query(_lib.Q_HEAD_WS, 4096, 10, 5) > 0
+  _check_head_and_plane_validation(built_lib)
+
+
+def _check_head_and_plane_validation(lib):
+  """Every check of the head, colsum and plane-GEMM entry points rejects its call with the right code and a message
+  naming the called function, before any launch: the pointers below are never dereferenced."""
+  import ctypes
+  from adanet_b200 import _lib
+  INVALID, UNSUPPORTED, WORKSPACE = -22, -95, -12
+  P, BIG = 1 << 20, 1 << 40           # fake device pointer / workspace size
+  members = _lib.ptr_array([P + 256 * k for k in range(64)])
+  gam = _lib.f32_array([0.5] * 64)
+  before = _lib.launch_count()
+
+  def rejects(name, want, phrase, *args):
+    rc = getattr(lib, name)(*args)
+    msg = lib.adn_last_error().decode()
+    assert (rc, phrase in msg, name in msg) == (want, True, True), (name, phrase, rc, msg)
+
+  def ens_head(want, phrase, **kw):
+    a = dict(head=0, mix=0, members=members, n=2, w=P, bias=None, gammas=gam, reg_is_zero=0, mult=1.0, labels=P,
+             labels_f=None, out3=P, dw=None, dbias=None, dens=None, ens_out=None, batch=256, dim=10, ws=P, ws_bytes=BIG)
+    a.update(kw)
+    rejects("adn_ensemble_head", want, phrase, *a.values(), None)
+
+  ens_head(INVALID, "null pointer", members=None)
+  ens_head(INVALID, "null pointer", out3=None)
+  ens_head(INVALID, "null pointer", ws=None)
+  ens_head(INVALID, "bad head", head=3)
+  ens_head(INVALID, "mixture type", mix=3)
+  ens_head(UNSUPPORTED, "n_members", n=0)
+  ens_head(UNSUPPORTED, "n_members", n=65)
+  ens_head(INVALID, "dw must be NULL", mix=_lib.MIX_MATRIX, dw=P)
+  ens_head(INVALID, "gammas missing", gammas=None)
+  ens_head(INVALID, "is null", members=_lib.ptr_array([P, None]))
+  ens_head(INVALID, "labels missing", labels=None)
+  ens_head(INVALID, "labels missing", head=_lib.HEAD_MSE)
+  ens_head(INVALID, "batch/dim", batch=0)
+  ens_head(UNSUPPORTED, "dim 65", dim=65)
+  ens_head(WORKSPACE, "workspace", ws_bytes=256)
+  ens_head(UNSUPPORTED, "shared memory", n=64, dim=64)
+
+  def head_loss(want, phrase, planes=False, **kw):
+    a = dict(head=0, logits=P, labels=P, labels_f=None, loss_out=P, dlogits=None)
+    a.update({k: kw.pop(k) for k in list(kw) if k in a})
+    if planes:
+      b = dict(planes=None, colsum=None, dz=0, batch=256, dim=10, ws=P, ws_bytes=BIG)
+      b.update(kw)
+      rejects("adn_head_loss_p", want, phrase, *a.values(), *b.values(), None)
+    else:
+      b = dict(batch=256, dim=10, ws=P, ws_bytes=BIG)
+      b.update(kw)
+      rejects("adn_head_loss", want, phrase, *a.values(), *b.values(), None)
+
+  for planes in (False, True):
+    head_loss(INVALID, "null pointer", planes, logits=None)
+    head_loss(INVALID, "null pointer", planes, loss_out=None)
+    head_loss(INVALID, "null pointer", planes, ws=None)
+    head_loss(INVALID, "bad head", planes, head=5)
+    head_loss(INVALID, "labels missing", planes, labels=None)
+    head_loss(INVALID, "batch/dim", planes, batch=0)
+    head_loss(UNSUPPORTED, "dim 65", planes, dim=65)
+    head_loss(WORKSPACE, "workspace", planes, ws_bytes=256)
+  head_loss(INVALID, "dz_log2_scale", True, dz=61)
+
+  def fwd_p(want, phrase, **kw):
+    a = dict(xp=P, wp=P, b=None, yp=P, y=None, batch=256, in_=64, out=32, act=0)
+    a.update(kw)
+    rejects("adn_dense_fwd_p", want, phrase, *a.values(), None)
+
+  fwd_p(INVALID, "null pointer", xp=None)
+  fwd_p(INVALID, "null pointer", wp=None)
+  fwd_p(INVALID, "exactly one of yp / y", y=P)
+  fwd_p(INVALID, "exactly one of yp / y", yp=None)
+  fwd_p(INVALID, "bad shape", batch=0)
+  fwd_p(INVALID, "bad shape", out=1 << 31)
+  fwd_p(INVALID, "bad act", act=7)
+
+  def bwd_p(want, phrase, **kw):
+    a = dict(xp=P, wp=P, dzp=P, dxp=None, dx=None, dx_colsum=None, dw=P, batch=256, in_=64, out=32, mask=1, dz=0,
+             ws=P, ws_bytes=BIG)
+    a.update(kw)
+    rejects("adn_dense_bwd_p", want, phrase, *a.values(), None)
+
+  bwd_p(INVALID, "null pointer", xp=None)
+  bwd_p(INVALID, "null pointer", dzp=None)
+  bwd_p(INVALID, "null pointer", ws=None)
+  bwd_p(INVALID, "wp required", wp=None, dxp=P)
+  bwd_p(INVALID, "at most one of dxp / dx", dxp=P, dx=P)
+  bwd_p(INVALID, "dx_colsum needs dx", dx_colsum=P)
+  bwd_p(INVALID, "bad shape", in_=0)
+  bwd_p(INVALID, "dz_log2_scale", dz=-61)
+
+  rejects("adn_colsum", INVALID, "null pointer", None, 256, 10, P, P, BIG, None)
+  rejects("adn_colsum", INVALID, "null pointer", P, 256, 10, P, None, BIG, None)
+  rejects("adn_colsum", INVALID, "bad shape", P, 0, 10, P, P, BIG, None)
+  rejects("adn_colsum", WORKSPACE, "workspace", P, 256, 10, P, P, 64 * 10 * 4 - 1, None)
+
+  def group(want, phrase, n=2, batch=256, dim=10, per_op=True, **kw):
+    ops = (_lib.HeadOp * 2)()
+    for o in ops:
+      o.head, o.mixture_type, o.n_members, o.reg_multiplier = 0, 0, 2, 1.0
+      o.members_host, o.gammas_host = ctypes.cast(members, ctypes.POINTER(ctypes.c_void_p)), gam
+      o.w, o.labels, o.out3, o.workspace, o.workspace_bytes = P, P, P, P, BIG
+    for k, v in kw.items():
+      setattr(ops[1], k, v)
+    rejects("adn_head_group", want, phrase, ops if n >= 0 else None, abs(n), batch, dim, None)
+    if kw and per_op:
+      assert "op 1" in lib.adn_last_error().decode()
+
+  group(INVALID, "bad ops", n=-1)
+  group(INVALID, "batch/dim", batch=0)
+  group(INVALID, "batch/dim", dim=65)
+  group(INVALID, "null pointer", workspace=None)
+  group(INVALID, "null pointer", out3=None)
+  group(INVALID, "bad head", head=3)
+  group(INVALID, "mixture type", mixture_type=-1)
+  group(UNSUPPORTED, "n_members", n_members=0)
+  group(UNSUPPORTED, "n_members", n_members=65)
+  group(INVALID, "dw must be NULL", mixture_type=_lib.MIX_MATRIX, dw=P)
+  group(INVALID, "gammas missing", gammas_host=None)
+  group(INVALID, "labels missing", labels=None)
+  group(INVALID, "dz_log2_scale", dz_log2_scale=61)
+  group(WORKSPACE, "workspace", workspace_bytes=256)
+  group(UNSUPPORTED, "shared memory", dim=64, per_op=False, n_members=64)
+  assert _lib.launch_count() == before
 
 
 def test_engine_fails_loudly_without_gpu():
