@@ -16,11 +16,14 @@ back-propagated gradient stays in plane format between GEMMs.  A step is a wave
 schedule (IterationPlan._enqueue_waves) of grouped launches built from one op
 builder per stage:
 
-  forward layer   -> DenseNet.fwd_op          in adn_dense_fwd_p_group (frozen members too)
+  forward layer   -> DenseNet.fwd_op          in adn_dense_fwd_p_group (frozen members too: _fwd_waves)
   losses, heads   -> CandidatePlan.sub_head_op / EnsembleHead.head_op in adn_head_group
   backward layer  -> CandidatePlan.bwd_op     in adn_dense_bwd_p_group
   optimizers      -> _Optimizer.op            in adn_opt_step_group
   EMA / trace     -> EnsembleHead.book        in adn_head_bookkeeping
+
+Evaluation (IterationPlan.eval_step, EnsembleEvalPlan) runs the same builders: its nets go through
+_forward_inference (the forward waves without dropout) and each ensemble through EnsembleHead.enqueue_eval.
 
 With ADN_DENSE_PATH=simt the fp32 CUDA-core ABI is used instead, as an on-device
 cross-check: each candidate runs its whole step op by op (adn_dense_fwd /
@@ -35,7 +38,7 @@ from __future__ import annotations
 
 import ctypes
 import math
-from dataclasses import dataclass, field
+from dataclasses import dataclass, field, replace
 from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
@@ -66,6 +69,22 @@ def accuracy_of(logits: torch.Tensor, labels: torch.Tensor) -> float:
   """Fraction of correct predictions (correct_of)."""
   correct, total = correct_of(logits, labels)
   return correct / total
+
+
+def _check_metric(metric: str, head: int):
+  """Refuses an Evaluator metric the engine does not compute for a head of kind `head` (_HEAD_KIND)."""
+  if metric not in EVAL_METRICS:
+    raise NotImplementedError("Evaluator metric %r is not computed by the B200 engine (supported: %s)" % (metric, ", ".join(EVAL_METRICS)))
+  if metric == "accuracy" and head == _lib.HEAD_MSE:
+    raise ValueError("accuracy is not an evaluation metric of a regression head")
+
+
+def _metric_value(metric: str, out3: torch.Tensor, ens_logits: Optional[torch.Tensor], labels: torch.Tensor, b: int) -> float:
+  """A metric that passed _check_metric, of one evaluated ensemble: adanet_loss or the mean loss from its out3 =
+  (loss, reg, adanet_loss), or the accuracy of the first b rows of its ensemble logits."""
+  if metric == "accuracy":
+    return accuracy_of(ens_logits[:b], labels[:b])
+  return float(out3[2 if metric == "adanet_loss" else 0].item())
 
 
 def _check_head_ws(rows: int, logits_dim: int, n_members: int, have: int):
@@ -150,6 +169,38 @@ def matrix_member_logits(lib, members, mwp, mw_logits, xp, sp: int, mw=None, mw_
                "adn_dense_fwd_p")
     if mw is not None:
       _lib.check(lib.adn_l1_norm(mw[k].data_ptr(), mw[k].numel(), mw_l1.data_ptr() + 4 * k, sp), "adn_l1_norm")
+
+
+def _split_x(lib, x: torch.Tensor, xp: Optional[torch.Tensor], nets, sp: int):
+  """The minibatch's planes feed first dense layers (and MATRIX weights of linear members); conv stems read x, so
+  nets that all have one skip the split."""
+  if xp is not None and any(not n.stem for n in nets):
+    _lib.check(lib.adn_planes_split(x.data_ptr(), x.shape[0], x.shape[1], xp.data_ptr(), sp), "adn_planes_split")
+
+
+def _fwd_waves(lib, fwd, sp: int):
+  """Layer waves: one grouped forward launch per layer index and distinct batch size, larger batches first.
+  `fwd`: (net, input planes, batch, step counter of a TRAIN-mode forward or None, first minibatch row) per net."""
+  for w in range(max((len(n.ws) for n, _, _, _, _ in fwd), default=0)):
+    for bsz in sorted({b for _, _, b, _, _ in fwd}, reverse=True):
+      ops = [n.fwd_op(w, xp, sd, r0) for n, xp, b, sd, r0 in fwd if b == bsz and w < len(n.ws)]
+      if ops:
+        _lib.check(lib.adn_dense_fwd_p_group((_lib.FwdOp * len(ops))(*ops), len(ops), bsz, sp),
+                   "adn_dense_fwd_p_group")
+
+
+def _forward_inference(lib, nets, x: torch.Tensor, xp: Optional[torch.Tensor], sp: int):
+  """The inference-mode forward (no dropout) of `nets` on the static batch x.  Plane path (xp given): x split into
+  xp, the conv stems, then the forward waves.  SIMT path: each net's adn_dense_fwd layers."""
+  if xp is None:
+    for n in nets:
+      n.forward(lib, x, sp)
+    return
+  _split_x(lib, x, xp, nets, sp)
+  for n in nets:
+    if n.stem:
+      n.stem_forward(lib, x, sp)
+  _fwd_waves(lib, [(n, xp, n.batch, None, 0) for n in nets], sp)
 
 
 def _select_prev(prev_mixture_weights, idx: List[int]):
@@ -478,16 +529,9 @@ class DenseNet:
     d = self.dropout[i] if (self.dropout and 0 <= i < len(self.dropout)) else None
     return 1.0 / (1.0 - float(d[0])) if d is not None else 1.0
 
-  def forward(self, lib, x: torch.Tensor, sp: int, xp: Optional[torch.Tensor] = None):
-    """x: dense fp32 minibatch; xp: its split planes (required on the plane path)."""
+  def forward(self, lib, x: torch.Tensor, sp: int):
+    """The fp32 SIMT forward of the dense fp32 minibatch x, layer by layer (the plane path runs fwd_op waves)."""
     n = len(self.ws)
-    if self.planes:
-      if self.stem:
-        self.stem_forward(lib, x, sp)
-      for i in range(n):
-        _lib.check(lib.adn_dense_fwd_p_group((_lib.FwdOp * 1)(self.fwd_op(i, xp)), 1, self.batch, sp),
-                   "adn_dense_fwd_p_group")
-      return
     h = x
     for i in range(n):
       act = _lib.ACT_RELU if i < n - 1 else _lib.ACT_NONE
@@ -532,6 +576,7 @@ class EnsembleHead:
     self.planes = planes_enabled()
     self.dz_log2 = grad_log2_scale(batch)
     self.kind = getattr(ens, "kind", "complexity_regularized")
+    trains = ens.optimizer is not None and self.kind != "mean"
     self.mix = _MIX_KIND[ens.mixture_weight_type]
     if self.mix == _lib.MIX_MATRIX:
       # W_k [D_k, C] (zeros, weighted.py:424-428) applied to each member's last layer by the plane GEMM; the
@@ -540,13 +585,15 @@ class EnsembleHead:
         raise NotImplementedError("MATRIX mixture weights run on the plane path only (ADN_DENSE_PATH=simt is a cross-check)")
       self.mw = [torch.zeros((m.last_layer_dim, logits_dim), **f32) for m in self.member_nets]
       self.mwp = [new_planes(m.last_layer_dim, logits_dim, device) for m in self.member_nets]
-      self.d_mw = [torch.zeros_like(w) for w in self.mw]
       self.mw_logits = [torch.empty((batch, logits_dim), **f32) for _ in self.member_nets]
       self.mw_l1 = torch.zeros((n_members,), **f32)
-      self.dens = torch.empty((batch, logits_dim), **f32)
-      self.densp = new_planes(batch, logits_dim, device)
-      self.mw_ws_bytes = max(_lib.query(_lib.Q_DENSE_BWD_P_WS, batch, m.last_layer_dim, logits_dim) for m in self.member_nets)
-      self.mw_ws = torch.empty((self.mw_ws_bytes,), dtype=torch.uint8, device=device)
+      if trains:
+        # what only the weight gradients read (enqueue_matrix)
+        self.d_mw = [torch.zeros_like(w) for w in self.mw]
+        self.dens = torch.empty((batch, logits_dim), **f32)
+        self.densp = new_planes(batch, logits_dim, device)
+        self.mw_ws_bytes = max(_lib.query(_lib.Q_DENSE_BWD_P_WS, batch, m.last_layer_dim, logits_dim) for m in self.member_nets)
+        self.mw_ws = torch.empty((self.mw_ws_bytes,), dtype=torch.uint8, device=device)
       self.mix_w = self.mw_l1
     else:
       wshape = (n_members,) if self.mix == _lib.MIX_SCALAR else (n_members, logits_dim)
@@ -594,7 +641,7 @@ class EnsembleHead:
     self.reg_multiplier = 1.0 if ens.legacy_train_op else 2.0   # SURVEY.md section 3.3 step 11
     self.out3 = alloc((3,))
     self.ens_opt = None
-    if ens.optimizer is not None and self.kind != "mean":
+    if trains:
       if self.mix == _lib.MIX_MATRIX:
         ens_params = list(self.mw) + ([self.bias] if ens.use_bias else [])
         self._ens_grads = list(self.d_mw) + ([self.d_bias] if ens.use_bias else [])
@@ -713,14 +760,22 @@ class EnsembleHead:
     out["trace"] = self.trace.cpu().numpy()
     return out
 
-  def load_state_dict(self, st: Dict[str, np.ndarray]):
-    for i, t in enumerate(self.mixture_weight_tensors()):
-      t.copy_(torch.as_tensor(st["mix%d" % i]))
+  def set_weights(self, mixture_weights: Sequence[np.ndarray], bias: np.ndarray):
+    """Writes the mixture weights (one array per mixture_weight_tensors() entry) and the bias; MATRIX weights are
+    re-split into their planes."""
+    tensors = self.mixture_weight_tensors()
+    if len(mixture_weights) != len(tensors):
+      raise ValueError("%s takes %d mixture weight tensors, got %d" % (self.name, len(tensors), len(mixture_weights)))
+    for t, w in zip(tensors, mixture_weights):
+      t.copy_(torch.as_tensor(w).reshape(t.shape))
     if self.mix == _lib.MIX_MATRIX:
       sp = torch.cuda.current_stream(self.device).cuda_stream
       for w, wp in zip(self.mw, self.mwp):
         _lib.check(self.lib.adn_planes_split(w.data_ptr(), w.shape[0], w.shape[1], wp.data_ptr(), sp), "adn_planes_split")
-    self.bias.copy_(torch.as_tensor(st["bias"]))
+    self.bias.copy_(torch.as_tensor(bias).reshape(self.bias.shape))
+
+  def load_state_dict(self, st: Dict[str, np.ndarray]):
+    self.set_weights([st["mix%d" % i] for i in range(len(self.mixture_weight_tensors()))], st["bias"])
     if self.ens_opt is not None:
       self.ens_opt.load_state({k[len("ens_opt_"):]: v for k, v in st.items() if k.startswith("ens_opt_")})
     self.ema_state.copy_(torch.as_tensor(st["ema_state"]))
@@ -1078,16 +1133,6 @@ class IterationPlan:
     st["pending"] = False
 
   # -- one step --------------------------------------------------------------
-  def _fwd_waves(self, fwd, sp: int):
-    """Layer waves: one grouped forward launch per layer index and distinct batch size, larger batches first.
-    `fwd`: (net, input planes, batch, step counter of a TRAIN-mode forward or None, first minibatch row) per net."""
-    for w in range(max((len(n.ws) for n, _, _, _, _ in fwd), default=0)):
-      for bsz in sorted({b for _, _, b, _, _ in fwd}, reverse=True):
-        ops = [n.fwd_op(w, xp, sd, r0) for n, xp, b, sd, r0 in fwd if b == bsz and w < len(n.ws)]
-        if ops:
-          _lib.check(self.lib.adn_dense_fwd_p_group((_lib.FwdOp * len(ops))(*ops), len(ops), bsz, sp),
-                     "adn_dense_fwd_p_group")
-
   def _bwd_waves(self, cands, xp_of, sp: int):
     """Backward waves of the candidates, logits layer first: one grouped launch per wave and distinct batch size.
     `xp_of(c)`: the input planes of candidate c."""
@@ -1117,7 +1162,7 @@ class IterationPlan:
                      "adn_planes_split")
         else:
           c.net.stem_forward(lib, c.x_own, sp)
-      self._fwd_waves([(c.net, c.xp_own, c.batch, self.step_dev, 0) for c in bag], sp)
+      _fwd_waves(lib, [(c.net, c.xp_own, c.batch, self.step_dev, 0) for c in bag], sp)
       own = self.labels is not None
       ops = [c.sub_head_op(c.labels_own if own else None, None if own else c.labels_own, c.own_out3) for c in bag]
       _lib.check(lib.adn_head_group((_lib.HeadOp * len(ops))(*ops), len(ops), self.batch, self.C, sp), "adn_head_group")
@@ -1127,7 +1172,7 @@ class IterationPlan:
           c.enqueue_stem_bwd(c.x_own, sp)
       oops = [c.sub_opt.op(c._grads) for c in bag]
       _lib.check(lib.adn_opt_step_group((_lib.OptOp * len(oops))(*oops), len(oops), sp), "adn_opt_step_group")
-    self._split_x(sp)
+    _split_x(lib, self.x, self.xp, list(self.frozen) + [c.net for c in self.candidates], sp)
     # a row-sharded candidate consumes its own slice of the minibatch rows
     for c in self.sharded:
       if c.xp_local is not None:
@@ -1143,8 +1188,8 @@ class IterationPlan:
         c.net.stem_forward(lib, x_of(c), sp)
     # whole candidates and frozen members run the full minibatch, row-sharded candidates their slice; candidates run
     # in TRAIN mode (dropout), a row-sharded one draws its rows of the whole minibatch's mask
-    self._fwd_waves([(f, self.xp, self.batch, None, 0) for f in self.frozen] +
-                    [(c.net, xp_of(c), c.batch, self.step_dev, c.row0) for c in self.candidates], sp)
+    _fwd_waves(lib, [(f, self.xp, self.batch, None, 0) for f in self.frozen] +
+               [(c.net, xp_of(c), c.batch, self.step_dev, c.row0) for c in self.candidates], sp)
     # steps 3 and 6-11 of every candidate in one grouped launch (+ one finalize): the subnetwork losses (dlogits planes,
     # logits-layer bias gradients) and every SCALAR / VECTOR candidate-ensemble head; MATRIX heads run their plane
     # GEMMs around their own head launch
@@ -1186,8 +1231,7 @@ class IterationPlan:
     lib = self.lib
     main = torch.cuda.current_stream(self.device)
     sp = main.cuda_stream
-    for f in self.frozen:   # shared by every candidate ensemble on this GPU
-      f.forward(lib, self.x, sp)
+    _forward_inference(lib, self.frozen, self.x, self.xp, sp)   # shared by every candidate ensemble on this GPU
     if self.multi_stream:
       for c, s in zip(self.candidates, self.streams):
         s.wait_stream(main)
@@ -1199,12 +1243,6 @@ class IterationPlan:
       for c in self.candidates:
         c.enqueue_simt_step(self.x, self.labels, self.labels_f, self.step_dev, sp)
     _lib.check(lib.adn_counter_add(self.step_dev.data_ptr(), 1, sp), "adn_counter_add")
-
-  def _split_x(self, sp: int):
-    # the minibatch's own planes feed first dense layers (and MATRIX weights of linear members); conv stems read x
-    if self.xp is not None and any(not n.stem for n in list(self.frozen) + [c.net for c in self.candidates]):
-      _lib.check(self.lib.adn_planes_split(self.x.data_ptr(), self.batch, self.in_dim, self.xp.data_ptr(), sp),
-                 "adn_planes_split")
 
   def train_step(self, x=None, y=None, own_batches: Optional[Dict[int, tuple]] = None):
     """One training step of every candidate on this GPU on one minibatch: the one passed in, or the one
@@ -1252,30 +1290,18 @@ class IterationPlan:
     head's mean loss over the b examples) or "accuracy" (classification heads; arg-max of the ensemble logits,
     sigmoid heads at 0).  The members run in inference mode (no dropout) at the static batch, a partial batch
     zero-padded; the heads read the first b rows."""
-    if metric not in EVAL_METRICS:
-      raise NotImplementedError("Evaluator metric %r is not computed by the B200 engine (supported: %s)" % (metric, ", ".join(EVAL_METRICS)))
-    if metric == "accuracy" and self.head == "mse":
-      raise ValueError("accuracy is not an evaluation metric of a regression head")
+    _check_metric(metric, _HEAD_KIND[self.head])
     if self.sharded:
       raise NotImplementedError("hold-out evaluation of row-sharded candidates: use placement='balanced' with an Evaluator")
     labels = self.labels if self.labels is not None else self.labels_f
     b = _load_rows(self.x, labels, x, y)
     sp = torch.cuda.current_stream(self.device).cuda_stream
-    self._split_x(sp)
-    for f in self.frozen:
-      f.forward(self.lib, self.x, sp, self.xp)
-    for c in self.candidates:
-      c.net.forward(self.lib, self.x, sp, self.xp)
-    out = []
-    ens_out = torch.empty((self.batch, self.C), dtype=torch.float32, device=self.device) if metric == "accuracy" else None
-    for _, h, _ in self.heads:
+    _forward_inference(self.lib, list(self.frozen) + [c.net for c in self.candidates], self.x, self.xp, sp)
+    ens_outs = [torch.empty((self.batch, self.C), dtype=torch.float32, device=self.device) if metric == "accuracy" else None
+                for _ in self.heads]
+    for (_, h, _), ens_out in zip(self.heads, ens_outs):
       h.enqueue_eval(self.labels, self.labels_f, ens_out, sp, self.xp, rows=b)
-      if metric == "accuracy":
-        out.append(accuracy_of(ens_out[:b], labels[:b]))
-    torch.cuda.current_stream(self.device).synchronize()
-    if metric == "accuracy":
-      return out
-    return [float(h.out3[2 if metric == "adanet_loss" else 0].item()) for _, h, _ in self.heads]
+    return [_metric_value(metric, h.out3, ens_out, labels, b) for (_, h, _), ens_out in zip(self.heads, ens_outs)]
 
   # -- in-flight checkpoint -------------------------------------------------------
   def state_dict(self) -> Dict[str, np.ndarray]:
@@ -1341,89 +1367,58 @@ class IterationPlan:
 
 
 class EnsembleEvalPlan:
-  """Forward-only evaluation of a finished ensemble (evaluate / predict and the
-  `previous_ensemble` candidate of the Evaluator): frozen members replayed with
-  adn_dense_fwd, then a one-op adn_head_group for logits and loss
-  (adanet/core/estimator.py:1785-1882 rebuilds the same thing as a TF graph)."""
+  """Forward-only evaluation of a finished ensemble (evaluate / predict and the `previous_ensemble` candidate of the
+  Evaluator): the members replayed by _forward_inference, then an EnsembleHead over them that holds the given weights
+  and trains nothing (adanet/core/estimator.py:1785-1882 rebuilds the same thing as a TF graph)."""
 
-  def __init__(self, members: Sequence[DenseNet], mix_w: np.ndarray, bias: np.ndarray, ens: EnsemblerPlanSpec,
+  def __init__(self, members: Sequence[DenseNet], mix_w, bias: np.ndarray, ens: EnsemblerPlanSpec,
                head: str, batch: int, logits_dim: int, device: Optional[torch.device] = None):
+    """`mix_w`: the SCALAR [N] / VECTOR [N, C] mixture weights, or the list of the N MATRIX W_k [D_k, C]."""
     self.lib = _require_cuda()
     self.device = device or torch.device("cuda", torch.cuda.current_device())
-    self.members, self.batch, self.C, self.head = list(members), batch, logits_dim, _HEAD_KIND[head]
-    self.fmt = _lib.plane_format()      # xp / mwp are sized for it: a plan outlives no format switch
-    for m in self.members:
+    self.batch, self.C = batch, logits_dim
+    self.fmt = _lib.plane_format()      # xp and the head's planes are sized for it: a plan outlives no format switch
+    for m in members:
       m.ensure_format()
       if m.batch != batch:
         raise ValueError("member %s was built for batch %d, eval plan uses %d" % (m.name, m.batch, batch))
+    # no optimizer (and no initializer call): the head allocates nothing that only training reads
+    self.head = EnsembleHead(self.lib, "ensemble", members, 0, replace(ens, optimizer=None, initial_weight_fn=None),
+                             batch, logits_dim, head, 0.0, 1, self.device)
+    self.head.set_weights(list(mix_w) if self.head.mix == _lib.MIX_MATRIX else [mix_w], bias)
+    self.out3 = self.head.out3
     f32 = dict(dtype=torch.float32, device=self.device)
-    self.mix = _MIX_KIND[ens.mixture_weight_type]
-    if self.mix == _lib.MIX_MATRIX:
-      # mix_w: list of [D_k, C] matrices; members are pre-multiplied by the plane GEMM, w = their L1 norms
-      if not planes_enabled():
-        raise NotImplementedError("MATRIX mixture weights run on the plane path only")
-      self.mw = [torch.as_tensor(np.ascontiguousarray(w, dtype=np.float32)).to(self.device) for w in mix_w]
-      self.mwp = [new_planes(w.shape[0], w.shape[1], self.device) for w in self.mw]
-      sp0 = torch.cuda.current_stream(self.device).cuda_stream
-      for w, wp in zip(self.mw, self.mwp):
-        _lib.check(self.lib.adn_planes_split(w.data_ptr(), w.shape[0], w.shape[1], wp.data_ptr(), sp0), "adn_planes_split")
-      self.mw_logits = [torch.empty((batch, logits_dim), **f32) for _ in self.mw]
-      self.mix_w = torch.as_tensor(np.array([np.abs(np.asarray(w, dtype=np.float32)).sum(dtype=np.float32)
-                                             for w in mix_w], dtype=np.float32)).to(self.device)
-    else:
-      self.mix_w = torch.as_tensor(np.ascontiguousarray(mix_w, dtype=np.float32)).to(self.device).reshape(
-          (len(members),) if self.mix == _lib.MIX_SCALAR else (len(members), logits_dim))
-    self.bias = torch.as_tensor(np.ascontiguousarray(bias, dtype=np.float32)).to(self.device)
-    lam, beta = float(ens.adanet_lambda), float(ens.adanet_beta)
-    self.reg_is_zero = int(lam == 0.0 and beta == 0.0)
-    self.gammas = gammas(lam, beta, [m.complexity for m in self.members])
-    self._gammas = _lib.f32_array(self.gammas)
-    self._members = _lib.ptr_array([t.data_ptr() for t in self.mw_logits] if self.mix == _lib.MIX_MATRIX
-                                   else [m.logits.data_ptr() for m in self.members])
-    self.out3 = torch.zeros((3,), **f32)
     self.ens_logits = torch.empty((batch, logits_dim), **f32)
     self.rows = 0             # examples of the last `run`: its logits are the first rows of ens_logits
-    self.ws_bytes = _lib.query(_lib.Q_HEAD_WS, batch, logits_dim, len(self.members))
-    self.workspace = torch.empty((self.ws_bytes,), dtype=torch.uint8, device=self.device)
     self.x = torch.empty((batch, members[0].in_dim), **f32)
     self.xp = new_planes(batch, members[0].in_dim, self.device) if planes_enabled() else None
     self.labels = torch.zeros((batch,), dtype=torch.int64, device=self.device) if head == "softmax_xent" else None
     self.labels_f = torch.zeros((batch, logits_dim), **f32) if head != "softmax_xent" else None
 
-  def run(self, x, y=None, forward_members: bool = True):
+  # the head's state under the plan's own names
+  members = property(lambda self: self.head.member_nets)
+  mix = property(lambda self: self.head.mix)
+  mix_w = property(lambda self: self.head.mix_w)
+  bias = property(lambda self: self.head.bias)
+  gammas = property(lambda self: self.head.gammas)
+  mw = property(lambda self: self.head.mw)
+  mwp = property(lambda self: self.head.mwp)
+  mw_logits = property(lambda self: self.head.mw_logits)
+
+  def run(self, x, y=None):
     """Evaluates the ensemble on the b <= batch examples of `x`: returns (loss, reg, adanet_loss) over them as
     floats (NaN-free only when labels given) and leaves their ensemble logits in the first b rows of
     `self.ens_logits` (`self.rows` = b).  The members run at the static batch, a partial batch zero-padded."""
     sp = torch.cuda.current_stream(self.device).cuda_stream
-    b = _load_rows(self.x, self.labels if self.labels is not None else self.labels_f, x, y)
-    self.rows = b
-    _check_head_ws(b, self.C, len(self.members), self.ws_bytes)
-    if forward_members:
-      if self.xp is not None and any(not m.stem for m in self.members):
-        _lib.check(self.lib.adn_planes_split(self.x.data_ptr(), self.batch, self.x.shape[1], self.xp.data_ptr(), sp),
-                   "adn_planes_split")
-      for m in self.members:
-        m.forward(self.lib, self.x, sp, self.xp)
-      if self.mix == _lib.MIX_MATRIX:
-        matrix_member_logits(self.lib, self.members, self.mwp, self.mw_logits, self.xp, sp)
-    op = _lib.HeadOp(self.head, self.mix, ctypes.cast(self._members, ctypes.POINTER(ctypes.c_void_p)), len(self.members),
-                     self.reg_is_zero, self.mix_w.data_ptr(), self.bias.data_ptr(),
-                     ctypes.cast(self._gammas, ctypes.POINTER(ctypes.c_float)), 1.0, 0,
-                     self.labels.data_ptr() if self.labels is not None else None,
-                     self.labels_f.data_ptr() if self.labels_f is not None else None, self.out3.data_ptr(), None, None,
-                     None, self.ens_logits.data_ptr(), None, 0, 0, self.workspace.data_ptr(), self.ws_bytes)
-    _run_head(self.lib, op, b, self.C, sp)
+    self.rows = _load_rows(self.x, self.labels if self.labels is not None else self.labels_f, x, y)
+    _forward_inference(self.lib, self.head.member_nets, self.x, self.xp, sp)
+    self.head.enqueue_eval(self.labels, self.labels_f, self.ens_logits, sp, self.xp, rows=self.rows)
     o = self.out3.cpu().numpy()
     return float(o[0]), float(o[1]), float(o[2])
 
   def metric(self, x, y, metric: str = "adanet_loss") -> float:
     """One Evaluator metric of the finished ensemble on a batch (see IterationPlan.eval_step)."""
-    if metric not in EVAL_METRICS:
-      raise NotImplementedError("Evaluator metric %r is not computed by the B200 engine (supported: %s)" % (metric, ", ".join(EVAL_METRICS)))
-    loss, _, adanet = self.run(x, y)
-    if metric == "accuracy":
-      if self.head == _lib.HEAD_MSE:
-        raise ValueError("accuracy is not an evaluation metric of a regression head")
-      b = self.rows
-      return accuracy_of(self.ens_logits[:b], (self.labels if self.labels is not None else self.labels_f)[:b])
-    return adanet if metric == "adanet_loss" else loss
+    _check_metric(metric, self.head.head)
+    self.run(x, y)
+    return _metric_value(metric, self.out3, self.ens_logits, self.labels if self.labels is not None else self.labels_f,
+                         self.rows)

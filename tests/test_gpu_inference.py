@@ -14,7 +14,8 @@ add 2 (N + 1) U of rounding to sum_k |w_k| E_k, and the head's loss bound follow
                     out3 within their bounds, `y=None` gives the same logits, a second run the same bytes, the members
                     are left byte-identical, and a partial batch evaluates its own rows
   eval_step         all four metrics of every candidate ensemble after two training steps, on a full and a partial
-                    batch; a dropout candidate evaluates without its mask; the training state is left byte-identical
+                    batch; a dropout candidate evaluates without its mask; the training state is left byte-identical;
+                    an EnsembleEvalPlan over a candidate ensemble's members and trained weights gives eval_step's bytes
   Estimator         evaluate / predict over an input with a ragged tail, against float64 of ensemble-latest.npz; a
                     fresh Estimator predicts the same bytes; an Evaluator with a ragged hold-out set ranks every
                     candidate and the previous ensemble by their float64 values
@@ -472,6 +473,56 @@ def test_eval_step_metrics(fmt, name):
   for key in before:
     if not np.array_equal(before[key], after[key], equal_nan=True):
       fails.append("eval_step changed %s" % key)
+  torch.cuda.synchronize()
+  assert not fails, "\n".join(fails[:30])
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("name", ["cnn", "vector_warm", "matrix", "shared"])
+def test_eval_plan_matches_eval_step(fmt, name, monkeypatch):
+  """An EnsembleEvalPlan built from a candidate ensemble's members and trained weights (what the Evaluator ranks as
+  the previous ensemble at the next iteration) gives the bytes eval_step gives for that ensemble: out3 and the
+  ensemble logits, on a full and a partial batch.  SCALAR (with a conv-stem member), VECTOR and MATRIX mixture
+  weights with lambda, beta != 0, and Solo / All / second-ensembler / MeanEnsembler heads."""
+  import torch
+  from adanet_b200 import _lib
+  from adanet_b200.core import engine as eng
+  from tests.test_gpu_step_state import _batch
+  case = dict(CASES[name], inject=None)
+  frozen, cands, warm = _case_data(case, seed=21)
+  plan, _ = _build_plan(case, frozen, cands, warm)
+  for k in range(2):
+    plan.train_step(*_batch(case, k))
+  evals = []
+  for _, h, _ in plan.heads:
+    w = [t.cpu().numpy() for t in h.mixture_weight_tensors()]
+    evals.append(eng.EnsembleEvalPlan(h.member_nets, w if h.mix == _lib.MIX_MATRIX else w[0], h.bias.cpu().numpy(), h.ens,
+                                      case["head"], case["B"], case["C"], plan.device))
+  seen = {}
+
+  def capture(h):
+    enqueue_eval = h.enqueue_eval
+
+    def wrapped(labels, labels_f, ens_out, sp, xp=None, rows=None):
+      enqueue_eval(labels, labels_f, ens_out, sp, xp, rows)
+      seen[id(h)] = (h.out3.clone(), ens_out[:rows].clone())
+    return wrapped
+
+  for _, h, _ in plan.heads:
+    monkeypatch.setattr(h, "enqueue_eval", capture(h))
+  fails = []
+  for rows in (case["B"], case["B"] // 2 + 1):
+    xe, ye = _batch(case, 99)
+    xe, ye = xe[:rows], ye[:rows]
+    plan.eval_step(xe, ye, "accuracy")
+    for (_, h, _), ev in zip(plan.heads, evals):
+      got3 = np.asarray(ev.run(xe, ye), dtype=np.float32)
+      out3, logits = seen[id(h)]
+      tag = "%s %s, %d rows" % (name, h.name, rows)
+      if got3.tobytes() != out3.cpu().numpy().tobytes():
+        fails.append("%s: the eval plan returns %r, eval_step's head holds %r" % (tag, got3, out3.cpu().numpy()))
+      if not _same_bytes([ev.ens_logits[:rows]], [logits]):
+        fails.append("%s: the eval plan's ensemble logits differ from eval_step's" % tag)
   torch.cuda.synchronize()
   assert not fails, "\n".join(fails[:30])
 
