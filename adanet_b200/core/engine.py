@@ -178,12 +178,36 @@ def _split_x(lib, x: torch.Tensor, xp: Optional[torch.Tensor], nets, sp: int):
     _lib.check(lib.adn_planes_split(x.data_ptr(), x.shape[0], x.shape[1], xp.data_ptr(), sp), "adn_planes_split")
 
 
+def _levels(nets) -> Dict[Tuple[int, int], int]:
+  """Dependency level of every layer of `nets`: 1 + the largest level of the layers it reads (its own previous layer
+  and the member layers of its pieces), 0 for a first layer on the input.  For a net without pieces it is the layer
+  index.  Keys are (id(net), layer)."""
+  known = {id(n) for n in nets}
+  level: Dict[Tuple[int, int], int] = {}
+
+  def of(n, i):
+    key = (id(n), i)
+    if key not in level:
+      for m, _ in n.producers(i):
+        if id(m) not in known:
+          raise RuntimeError("subnetwork %s reads %s, which is not run in the same forward pass" % (n.name, m.name))
+      level[key] = 1 + max((of(m, j) for m, j in n.producers(i)), default=-1)
+    return level[key]
+
+  for n in nets:
+    for i in range(len(n.ws)):
+      of(n, i)
+  return level
+
+
 def _fwd_waves(lib, fwd, sp: int):
-  """Layer waves: one grouped forward launch per layer index and distinct batch size, larger batches first.
-  `fwd`: (net, input planes, batch, step counter of a TRAIN-mode forward or None, first minibatch row) per net."""
-  for w in range(max((len(n.ws) for n, _, _, _, _ in fwd), default=0)):
+  """Layer waves: one grouped forward launch per dependency level (_levels) and distinct batch size, larger batches
+  first.  `fwd`: (net, input planes, batch, step counter of a TRAIN-mode forward or None, first minibatch row) per net."""
+  level = _levels([n for n, _, _, _, _ in fwd])
+  for w in range(max(level.values(), default=-1) + 1):
     for bsz in sorted({b for _, _, b, _, _ in fwd}, reverse=True):
-      ops = [n.fwd_op(w, xp, sd, r0) for n, xp, b, sd, r0 in fwd if b == bsz and w < len(n.ws)]
+      ops = [n.fwd_op(i, xp, sd, r0) for n, xp, b, sd, r0 in fwd if b == bsz
+             for i in range(len(n.ws)) if level[(id(n), i)] == w]
       if ops:
         _lib.check(lib.adn_dense_fwd_p_group((_lib.FwdOp * len(ops))(*ops), len(ops), bsz, sp),
                    "adn_dense_fwd_p_group")
@@ -297,6 +321,22 @@ class SubnetworkPlanSpec:
   last_layer_is_logits: bool = False
   # tf.layers.dropout after hidden layers in TRAIN mode (simple_dnn.py:80-81): per hidden layer (rate, seed) or None
   dropout: Optional[list] = None
+  # dense layers over graph.concat (core/lowering.py): per dense layer its pieces in concat order, or None for a plain
+  # layer; None = a plain chain.  A piece is {"src": "own" | "input" | "member", "rows": [r0, r1]} (+ "iteration",
+  # "name", "layer" of a previous-iteration member's hidden layer): "own" is the layer's primary piece -- its own
+  # previous layer, the input features for the first -- and the only one that receives dX; the kernel ws[i] is
+  # [sum of piece widths, out], its row blocks in piece order.  dims[i] is the primary piece's width.
+  inputs: Optional[list] = None
+
+
+def member_refs(inputs) -> List[Tuple[int, str]]:
+  """(iteration, name) of every previous-iteration member a piece list (SubnetworkPlanSpec.inputs) reads."""
+  return [(p["iteration"], p["name"]) for ps in (inputs or []) for p in (ps or []) if p["src"] == "member"]
+
+
+def extra_pieces(inputs, i: int) -> bool:
+  """True when dense layer i reads more than its primary piece."""
+  return bool(inputs) and i < len(inputs) and inputs[i] is not None and len(inputs[i]) > 1
 
 
 @dataclass
@@ -398,11 +438,22 @@ class DenseNet:
 
   def __init__(self, name: str, dims: Sequence[int], ws, bs, complexity: float, batch: int,
                device: torch.device, iteration: int = 0, shared: Optional[dict] = None,
-               image_shape: Optional[Sequence[int]] = None, dropout: Optional[list] = None):
+               image_shape: Optional[Sequence[int]] = None, dropout: Optional[list] = None,
+               inputs: Optional[list] = None, members: Sequence["DenseNet"] = ()):
     """`dropout`: per hidden layer (rate, seed) or None -- applied only by `fwd_op(..., step_dev=...)`, i.e. on the
-    TRAIN-mode forward of a candidate; frozen members and evaluation replay without it (iteration.py:568-579)."""
+    TRAIN-mode forward of a candidate; frozen members and evaluation replay without it (iteration.py:568-579).
+    `inputs`: the pieces of each dense layer (SubnetworkPlanSpec.inputs); their members are resolved by (iteration,
+    name) against `members`."""
     self.name, self.dims, self.complexity, self.iteration = name, list(dims), float(complexity), iteration
     self.dropout = list(dropout) if dropout else None
+    self._srcs: Dict[int, object] = {}      # fwd_op's piece arrays, kept alive while an op built from them is in use
+    self.inputs = [list(ps) if ps else None for ps in inputs] if inputs else None
+    by_key = {(m.iteration, m.name): m for m in members}
+    for key in member_refs(self.inputs):
+      if tuple(key) not in by_key:
+        raise NotImplementedError("subnetwork %s reads a hidden layer of %s (iteration %d), which is not a member of the "
+                                  "ensemble it is built with" % (name, key[1], key[0]))
+    self.members = {tuple(k): by_key[tuple(k)] for k in member_refs(self.inputs)}
     self.shared = shared or {}
     self.batch = batch
     self.device = device
@@ -427,18 +478,21 @@ class DenseNet:
     self.in_dim = int(np.prod(self.image_shape)) if self.stem else self.dims[0]
     self.fmt = _lib.plane_format()
     assert len(ws) == len(dims) - 1
+    if self.inputs is not None and len(self.inputs) != len(ws):
+      raise ValueError("subnetwork %s has %d dense layers but pieces for %d" % (name, len(ws), len(self.inputs)))
     self.ws = [torch.as_tensor(np.ascontiguousarray(w, dtype=np.float32)).to(device) for w in ws]
     self.bs = [torch.as_tensor(np.ascontiguousarray(b, dtype=np.float32)).to(device) for b in bs]
     for i, w in enumerate(self.ws):
-      if tuple(w.shape) != (dims[i], dims[i + 1]):
-        raise ValueError("kernel %d of %s has shape %s, want %s" % (i, name, tuple(w.shape), (dims[i], dims[i + 1])))
+      rows = self.piece_rows(i)
+      if tuple(w.shape) != (rows[-1][1], dims[i + 1]) or rows[self.primary(i)][1] - rows[self.primary(i)][0] != dims[i]:
+        raise ValueError("kernel %d of %s has shape %s, want %s" % (i, name, tuple(w.shape), (rows[-1][1], dims[i + 1])))
     self.planes = planes_enabled()
     n = len(self.ws)
     if self.planes:
       # hidden activations live as split planes; only the logits are dense fp32
       self.acts = [None] * (n - 1) + [torch.empty((batch, dims[-1]), dtype=torch.float32, device=device)]
       self.hp = [new_planes(batch, d, device) for d in dims[1:-1]]
-      self.wps = [new_planes(dims[i], dims[i + 1], device) for i in range(n)]
+      self._new_weight_planes()
       self.refresh_planes()
       self.fwd_ws_bytes, self.fwd_ws = 0, None
     else:
@@ -454,9 +508,8 @@ class DenseNet:
     if not self.planes or self.fmt == _lib.plane_format():
       return
     self.fmt = _lib.plane_format()
-    n = len(self.ws)
     self.hp = [new_planes(self.batch, d, self.device) for d in self.dims[1:-1]]
-    self.wps = [new_planes(self.dims[i], self.dims[i + 1], self.device) for i in range(n)]
+    self._new_weight_planes()
     if self.stem:
       self.stem_out = new_planes(self.batch, self.dims[0], self.device)
     self.refresh_planes()
@@ -468,8 +521,43 @@ class DenseNet:
       return
     sp = torch.cuda.current_stream(self.device).cuda_stream
     lib = _lib.load()
-    for w, wp in zip(self.ws, self.wps):
-      _lib.check(lib.adn_planes_split(w.data_ptr(), w.shape[0], w.shape[1], wp.data_ptr(), sp), "adn_planes_split")
+    for i, w in enumerate(self.ws):
+      for (r0, r1), wp in zip(self.piece_rows(i), self.piece_wps[i]):
+        _lib.check(lib.adn_planes_split(w[r0:r1].data_ptr(), r1 - r0, w.shape[1], wp.data_ptr(), sp), "adn_planes_split")
+
+  # ---- dense layers over a concat (SubnetworkPlanSpec.inputs) ----
+  def pieces(self, i: int) -> list:
+    """The pieces of dense layer i (a plain layer: its one primary piece)."""
+    if self.inputs is not None and self.inputs[i]:
+      return self.inputs[i]
+    return [{"src": "own", "rows": [0, self.dims[i]]}]
+
+  def piece_rows(self, i: int) -> List[Tuple[int, int]]:
+    return [(int(p["rows"][0]), int(p["rows"][1])) for p in self.pieces(i)]
+
+  def primary(self, i: int) -> int:
+    """Index of layer i's primary piece (its own previous layer / the input features) in its piece list."""
+    return next(k for k, p in enumerate(self.pieces(i)) if p["src"] == "own")
+
+  def _new_weight_planes(self):
+    """One plane tensor per piece of every kernel, each zero-padded in its own K tail; wps[i] is the primary one."""
+    self.piece_wps = [[new_planes(r1 - r0, self.dims[i + 1], self.device) for r0, r1 in self.piece_rows(i)]
+                      for i in range(len(self.ws))]
+    self.wps = [self.piece_wps[i][self.primary(i)] for i in range(len(self.ws))]
+
+  def piece_input(self, i: int, k: int, xp: Optional[torch.Tensor]) -> torch.Tensor:
+    """Input planes of piece k of layer i, taken from the referenced net now (its buffers change on a format switch)."""
+    p = self.pieces(i)[k]
+    if p["src"] == "own":
+      return (self.stem_out if self.stem else xp) if i == 0 else self.hp[i - 1]
+    if p["src"] == "input":
+      return xp
+    return self.members[(p["iteration"], p["name"])].hp[p["layer"]]
+
+  def producers(self, i: int) -> List[Tuple["DenseNet", int]]:
+    """(net, layer) whose forward output layer i reads: its own layer i - 1 and the members' layers of its pieces."""
+    out = [(self, i - 1)] if i > 0 else []
+    return out + [(self.members[(p["iteration"], p["name"])], p["layer"]) for p in self.pieces(i) if p["src"] == "member"]
 
   @property
   def logits(self) -> torch.Tensor:
@@ -517,6 +605,13 @@ class DenseNet:
     op = _lib.FwdOp(src.data_ptr(), self.wps[i].data_ptr(), self.bs[i].data_ptr(),
                     None if last else self.hp[i].data_ptr(), self.acts[i].data_ptr() if last else None,
                     self.dims[i], self.dims[i + 1], _lib.ACT_NONE if last else _lib.ACT_RELU, 0)
+    if extra_pieces(self.inputs, i):
+      rows, pk = self.piece_rows(i), self.primary(i)
+      extra = [k for k in range(len(rows)) if k != pk]
+      srcs = (_lib.FwdSrc * len(extra))(*[_lib.FwdSrc(self.piece_input(i, k, xp).data_ptr(), self.piece_wps[i][k].data_ptr(),
+                                                       rows[k][1] - rows[k][0]) for k in extra])
+      self._srcs[i] = srcs
+      op.srcs, op.n_srcs = ctypes.cast(srcs, ctypes.POINTER(_lib.FwdSrc)), len(extra)
     d = self.dropout[i] if (self.dropout and step_dev is not None and not last and i < len(self.dropout)) else None
     if d is not None:
       op.dropout_rate, op.dropout_seed, op.dropout_layer = float(d[0]), int(d[1]) & 0xffffffff, i
@@ -531,6 +626,8 @@ class DenseNet:
 
   def forward(self, lib, x: torch.Tensor, sp: int):
     """The fp32 SIMT forward of the dense fp32 minibatch x, layer by layer (the plane path runs fwd_op waves)."""
+    if self.inputs is not None:
+      raise NotImplementedError("subnetworks that read other subnetworks' hidden layers run on the plane path only")
     n = len(self.ws)
     h = x
     for i in range(n):
@@ -547,6 +644,16 @@ class DenseNet:
     if self.stem:
       ws, bs = [self.stem_k.cpu().numpy()] + ws, [self.stem_b.cpu().numpy()] + bs
     return ws, bs
+
+
+def check_matrix_members(nets):
+  """MATRIX mixture weights multiply a member's last layer; one whose logits layer reads a concat has the concat as its
+  last layer, which the engine does not multiply."""
+  for n in nets:
+    if extra_pieces(n.inputs, len(n.dims) - 2):
+      raise NotImplementedError("MATRIX mixture weights over subnetwork %s, whose last_layer is a concat with the hidden "
+                                "layers of other subnetworks, are not implemented by the B200 engine; use SCALAR or "
+                                "VECTOR" % n.name)
 
 
 class EnsembleHead:
@@ -581,6 +688,7 @@ class EnsembleHead:
     if self.mix == _lib.MIX_MATRIX:
       # W_k [D_k, C] (zeros, weighted.py:424-428) applied to each member's last layer by the plane GEMM; the
       # head kernel then sees pre-multiplied members and the L1 norms (include/adanet_b200.h)
+      check_matrix_members(self.member_nets)
       if not self.planes:
         raise NotImplementedError("MATRIX mixture weights run on the plane path only (ADN_DENSE_PATH=simt is a cross-check)")
       self.mw = [torch.zeros((m.last_layer_dim, logits_dim), **f32) for m in self.member_nets]
@@ -817,14 +925,19 @@ class CandidatePlan:
       raise NotImplementedError("MATRIX mixture weights over a subnetwork whose last_layer is its logits (%s) are not "
                                 "implemented by the B200 engine; pass last_layer_fn or use SCALAR / VECTOR" % spec.name)
     self.net = DenseNet(spec.name, spec.dims, spec.ws, spec.bs, spec.complexity, batch, device, iteration,
-                        spec.shared, spec.image_shape, dropout=getattr(spec, "dropout", None))
+                        spec.shared, spec.image_shape, dropout=getattr(spec, "dropout", None),
+                        inputs=getattr(spec, "inputs", None), members=frozen)
     if self.net.dropout and not self.net.planes:
       raise NotImplementedError("dropout runs on the plane path only")
     self.frozen = list(frozen)
     dims = self.net.dims
     f32 = dict(dtype=torch.float32, device=device)
-    # gradients and backward scratch
-    self.dws = [galloc(w.shape) for w in self.net.ws]
+    # gradients and backward scratch; a layer over a concat has one dW tensor per piece (piece_dws, concat order)
+    # instead of dws[i], each allocated on its own
+    net = self.net
+    self.piece_dws = [[galloc((r1 - r0, dims_i)) for r0, r1 in net.piece_rows(i)] if extra_pieces(net.inputs, i) else None
+                      for i, dims_i in enumerate(net.dims[1:])]
+    self.dws = [galloc(w.shape) if self.piece_dws[i] is None else None for i, w in enumerate(self.net.ws)]
     self.dbs = [galloc(b.shape) for b in self.net.bs]
     self.dlogits = torch.empty((batch, dims[-1]), **f32)
     hid = max(dims[1:-1]) if len(dims) > 2 else 0
@@ -838,6 +951,11 @@ class CandidatePlan:
       bwd_ws = max(_lib.query(_lib.Q_DENSE_BWD_P_WS, batch, dims[i], dims[i + 1]) for i in range(len(dims) - 1))
       self.bwd_ws_bytes = max(bwd_ws, _lib.query(_lib.Q_COLSUM_WS, batch, dims[-1]))
       self.bwd_ws = torch.empty((self.bwd_ws_bytes,), dtype=torch.uint8, device=device)
+      # every dW-only op of an extra piece carves its split-K partials from a workspace of its own
+      self.piece_ws = [[torch.empty((_lib.query(_lib.Q_DENSE_BWD_P_WS, batch, r1 - r0, dims[i + 1]),), dtype=torch.uint8,
+                                    device=device) if k != net.primary(i) else None
+                        for k, (r0, r1) in enumerate(net.piece_rows(i))] if self.piece_dws[i] is not None else None
+                       for i in range(len(dims) - 1)]
       ws_bytes = 0                    # `workspace` serves the subnetwork's own head op alone
     else:
       self.dz = [torch.empty((batch, hid), **f32) for _ in range(2)] if hid else []
@@ -871,6 +989,12 @@ class CandidatePlan:
       self._grads += [self.d_stem_k, self.d_stem_b]
       planes += [None, None]
     for i, (w, b, dw, db) in enumerate(zip(self.net.ws, self.net.bs, self.dws, self.dbs)):
+      if self.piece_dws[i] is not None:
+        # each piece is its own parameter: the kernel's row block (a contiguous view), its dW and its planes
+        params += [w[r0:r1] for r0, r1 in self.net.piece_rows(i)] + [b]
+        self._grads += list(self.piece_dws[i]) + [db]
+        planes += list(self.net.piece_wps[i]) + [None]
+        continue
       params += [w, b]
       self._grads += [dw, db]
       planes += [self.net.wps[i] if self.planes else None, None]
@@ -977,11 +1101,29 @@ class CandidatePlan:
     dx = self.dpool if (i == 0 and net.stem) else None
     # hidden activation i - 1 (the input of this layer) may have been dropped out: its sign bits already carry the keep
     # mask, the 1 / (1 - rate) factor rides on dx
+    dw = self.dws[i] if self.piece_dws[i] is None else self.piece_dws[i][net.primary(i)]
     return _lib.BwdOp(xin.data_ptr(), net.wps[i].data_ptr(), dzp.data_ptr(),
                       dxp.data_ptr() if dxp is not None else None, dx.data_ptr() if dx is not None else None,
-                      self.dbs[i - 1].data_ptr() if i > 0 else None, self.dws[i].data_ptr(), net.dims[i],
+                      self.dbs[i - 1].data_ptr() if i > 0 else None, dw.data_ptr(), net.dims[i],
                       net.dims[i + 1], 1 if (i > 0 or dx is not None) else 0, self.dz_log2, ws.data_ptr(),
                       self.bwd_ws_bytes, net.dx_mul(i - 1) if i > 0 else 0.0, 0.0)
+
+  def piece_bwd_ops(self, k: int, xp: torch.Tensor) -> List["_lib.BwdOp"]:
+    """The dW-only ops of the k-th backward wave's extra pieces (no wp, no dx), one per piece with its own dW and
+    workspace; they run in the same grouped launch as bwd_op(k)."""
+    net, n = self.net, len(self.net.ws)
+    i = n - 1 - k
+    if self.piece_dws[i] is None:
+      return []
+    dzp = self.dzp_out if k == 0 else self.dzp[(i + 1) % 2]
+    ops = []
+    for q, (r0, r1) in enumerate(net.piece_rows(i)):
+      if q != net.primary(i):
+        ws = self.piece_ws[i][q]
+        ops.append(_lib.BwdOp(net.piece_input(i, q, xp).data_ptr(), None, dzp.data_ptr(), None, None, None,
+                              self.piece_dws[i][q].data_ptr(), r1 - r0, net.dims[i + 1], 0, self.dz_log2, ws.data_ptr(),
+                              ws.numel(), 0.0, 0.0))
+    return ops
 
   def enqueue_stem_bwd(self, x: torch.Tensor, sp: int):
     """Kernel / bias gradients of the conv stem from the pooled-feature gradient the last backward wave left."""
@@ -990,6 +1132,40 @@ class CandidatePlan:
                                           self.d_stem_k.data_ptr(), self.d_stem_b.data_ptr(), self.batch, st["h"], st["w"],
                                           st["cin"], st["f"], self.stem_ws.data_ptr(), self.stem_ws_bytes, sp),
                "adn_conv_stem_bwd")
+
+
+def _check_connected(specs, idx, frozen, ens, ensemble_candidates, shards):
+  """Refuses, before anything is allocated or launched, the candidates that read other subnetworks' hidden layers in a
+  way the engine does not run."""
+  keys = {(f.iteration, f.name) for f in frozen}
+  if not planes_enabled() and any(f.inputs is not None for f in frozen):
+    raise NotImplementedError("frozen subnetworks that read other subnetworks' hidden layers run on the plane path only "
+                              "(not with ADN_DENSE_PATH=simt)")
+  matrix = ens.mixture_weight_type == "matrix" or any(
+      len(ec) > 4 and ec[4] is not None and ec[4].mixture_weight_type == "matrix" for ec in (ensemble_candidates or []))
+  if matrix:
+    for f in frozen:
+      if extra_pieces(f.inputs, len(f.dims) - 2):
+        raise NotImplementedError("MATRIX mixture weights over subnetwork %s, whose last_layer is a concat with the "
+                                  "hidden layers of other subnetworks, are not implemented by the B200 engine" % f.name)
+  for i, s in zip(idx, specs):
+    inputs = getattr(s, "inputs", None)
+    if inputs is None:
+      continue
+    what = "subnetwork %s reads the hidden layers of other subnetworks" % s.name
+    if not planes_enabled():
+      raise NotImplementedError(what + ": it runs on the plane path only (not with ADN_DENSE_PATH=simt)")
+    if i in shards:
+      raise NotImplementedError(what + ": it cannot be row-sharded (use placement='balanced')")
+    if getattr(s, "own_input", False):
+      raise NotImplementedError(what + ": it cannot be bagged on its own train_input_fn (the frozen hidden layers are "
+                                "those of the shared minibatch)")
+    if matrix and extra_pieces(inputs, len(s.dims) - 2):
+      raise NotImplementedError(what + " at its logits layer, so its last_layer is a concat: MATRIX mixture weights over "
+                                "it are not implemented by the B200 engine; use SCALAR or VECTOR")
+    for key in member_refs(inputs):
+      if tuple(key) not in keys:
+        raise NotImplementedError(what + ": %s (iteration %d) is not a frozen member of this iteration" % (key[1], key[0]))
 
 
 class IterationPlan:
@@ -1013,13 +1189,14 @@ class IterationPlan:
     self.lib = _require_cuda()
     self.device = device or torch.device("cuda", torch.cuda.current_device())
     self.iteration, self.batch, self.in_dim, self.C, self.head = iteration, batch, in_dim, logits_dim, head
+    idx = list(candidate_indices) if candidate_indices is not None else list(range(len(specs)))
+    _check_connected(specs, idx, frozen, ens, ensemble_candidates, shards or {})
     self.frozen = list(frozen)
     self.fmt = _lib.plane_format()
     for f in self.frozen:
       f.ensure_format()
       if f.batch != batch:
         raise ValueError("frozen member %s was built for batch %d, plan uses %d" % (f.name, f.batch, batch))
-    idx = list(candidate_indices) if candidate_indices is not None else list(range(len(specs)))
     warm = lambda e: prev_ens_name is None or prev_ens_name == e.name
     shards = shards or {}
     for i in idx:
@@ -1138,7 +1315,8 @@ class IterationPlan:
     `xp_of(c)`: the input planes of candidate c."""
     for k in range(max((len(c.net.ws) for c in cands), default=0)):
       for bsz in sorted({c.batch for c in cands}, reverse=True):
-        ops = [c.bwd_op(k, xp_of(c)) for c in cands if c.batch == bsz and k < len(c.net.ws)]
+        ops = [op for c in cands if c.batch == bsz and k < len(c.net.ws)
+               for op in [c.bwd_op(k, xp_of(c))] + c.piece_bwd_ops(k, xp_of(c))]
         if ops:
           _lib.check(self.lib.adn_dense_bwd_p_group((_lib.BwdOp * len(ops))(*ops), len(ops), bsz, sp),
                      "adn_dense_bwd_p_group")

@@ -272,7 +272,7 @@ class Estimator(object):
     for b in builders:
       spec, sub = lowering.build_and_lower(b, placeholders, labels_ph, self._head, iteration_step=0,
                                            previous_ensemble=self._previous_ensemble, in_dim=self._in_dim,
-                                           config=self._config)
+                                           config=self._config, iteration=iteration_number)
       specs.append(spec)
       subs.append(sub)
     if self._replicate_ensemble_in_training and any(sp.dropout and any(d is not None for d in sp.dropout) for sp in specs):
@@ -461,13 +461,18 @@ class Estimator(object):
       if _lib.plane_format() != _lib.PLANES_TF32:
         logging.info("model_dir %s was trained on TF32 planes: switching to them", self._model_dir)
         _lib.set_plane_format(_lib.PLANES_TF32)
+    from adanet_b200.core import lowering
+    dims_of = {(int(m["iteration"]), m["name"]): m["dims"] for m in meta["members"]}
+    dims_of = lambda it, name, _d=dims_of: _d[(int(it), name)]
     members = []
     for k, m in enumerate(meta["members"]):
       n_layers = len(m["dims"]) - 1 + (1 if m.get("image_shape") else 0)     # a conv stem's kernel / bias come first
       ws = [data["m{}_w{}".format(k, i)] for i in range(n_layers)]
       bs = [data["m{}_b{}".format(k, i)] for i in range(n_layers)]
+      # a member reads only members before it (the order the ensemble grew in)
       members.append(eng.DenseNet(m["name"], m["dims"], ws, bs, m["complexity"], s.batch, s.device, m["iteration"],
-                                  m["shared"], m.get("image_shape")))
+                                  lowering.decode_tensors(m["shared"], dims_of, s.in_dim), m.get("image_shape"),
+                                  inputs=m.get("inputs"), members=list(members)))
     s.frozen = members
     s.iteration = int(meta["iteration"])
     s.architecture = [(int(t), n) for t, n in meta["architecture"]]
@@ -486,9 +491,8 @@ class Estimator(object):
     self._member_subnetworks, self._member_builders, ws_list = [], [], []
     mw = s.mixture_weights
     for k, m in enumerate(meta["members"]):
-      lg = graph.placeholder(s.C, "restored_logits_{}".format(k))
-      sub = subnetwork_lib.Subnetwork(last_layer=graph.placeholder(m["dims"][-2], "restored_last_layer_{}".format(k)),
-                                      logits=lg, complexity=m["complexity"], shared=m["shared"])
+      sub = lowering.restored_subnetwork(m, dims_of, s.in_dim)
+      lg = sub.logits
       self._member_subnetworks.append(sub)
       self._member_builders.append(_RestoredBuilder(m["name"]))
       ws_list.append(ensemble_lib.WeightedSubnetwork(name=m["name"], iteration_number=m["iteration"],
@@ -708,6 +712,7 @@ class Estimator(object):
         out["mixture_weight_{}".format(k)] = w
     else:
       out["mixture_weights"] = s.mixture_weights
+    from adanet_b200.core import lowering
     for k, m in enumerate(s.frozen):
       ws, bs = m.numpy_params()
       for i, (w, b) in enumerate(zip(ws, bs)):
@@ -727,14 +732,27 @@ class Estimator(object):
         "prev_best_ema": None if s.prev_best_ema is None else float(s.prev_best_ema),
         "last_candidate_name": self._last_candidate_name, "winner_ens_index": int(s.winner_ens_index),
         "plane_format": "tf32" if fmt == _lib.PLANES_TF32 else "fp16",
-        "members": [{"name": m.name, "iteration": int(m.iteration), "complexity": float(m.complexity),
-                     "dims": [int(d) for d in m.dims], "shared": m.shared,
-                     "image_shape": list(m.image_shape) if m.stem else None} for m in s.frozen],
+        "members": [self._member_record(k, m, lowering) for k, m in enumerate(s.frozen)],
     }
     tmp = os.path.join(self._model_dir, "ensemble-latest.json.tmp")
     with open(tmp, "w") as f:
       json.dump(meta, f)
     os.replace(tmp, os.path.join(self._model_dir, "ensemble-latest.json"))
+
+  def _member_record(self, k, m, lowering):
+    """A frozen member's entry in ensemble-latest.json.  Tensors in `shared` are saved as references to the layers
+    they are (lowering.encode_tensors); a member over a concat adds its pieces ("inputs"), and one whose
+    persisted_tensors hold tensors adds those."""
+    rec = {"name": m.name, "iteration": int(m.iteration), "complexity": float(m.complexity),
+           "dims": [int(d) for d in m.dims], "shared": lowering.encode_tensors(m.shared),
+           "image_shape": list(m.image_shape) if m.stem else None}
+    if m.inputs is not None:
+      rec["inputs"] = m.inputs
+    subs = getattr(self, "_member_subnetworks", None) or []
+    pt = subs[k].persisted_tensors if k < len(subs) else None
+    if pt and lowering.encode_tensors(pt) is not pt:
+      rec["persisted_tensors"] = lowering.encode_tensors(pt)
+    return rec
 
   # ------------------------------------------------------------------ evaluate / predict
   def _restore_for_inference(self, input_fn):

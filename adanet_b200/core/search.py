@@ -164,6 +164,7 @@ class AdaNetSearch:
       raise ValueError("the ensemble strategies produced no candidate")
     if len(self.ensemblers) > 1:      # strategy candidates x ensemblers, strategy-candidate major (iteration.py:683-693)
       ecs = [EnsembleCandidate(c.name, list(c.builders), c.keep_previous, j) for c in ecs for j in range(len(self.ensemblers))]
+    self._check_kept_members(specs, ecs)
     self._ecands = ecs
     # subnetwork -> rank.  Subnetworks read by the same candidate ensemble (e.g. AllStrategy) must share a GPU --
     # splitting them would need the member logits gathered every step (SURVEY.md 8e) -- so the units of placement
@@ -205,6 +206,19 @@ class AdaNetSearch:
                                   prev_bias=self.bias, ensemble_candidates=local, prev_ens_name=prev_ens_name,
                                   shards=shards)
     return self.plan
+
+  def _check_kept_members(self, specs, ecs):
+    """A candidate ensemble must keep every previous member that its new subnetworks, or the members it keeps, read:
+    the winner's members are replayed from that list alone."""
+    for c in ecs:
+      kept = [self.frozen[i] for i in eng.kept_indices(c.keep_previous, len(self.frozen))]
+      keys = {(f.iteration, f.name) for f in kept}
+      reads = [(specs[b].name, key) for b in c.builders for key in eng.member_refs(getattr(specs[b], "inputs", None))]
+      reads += [(f.name, key) for f in kept for key in eng.member_refs(f.inputs)]
+      for who, key in reads:
+        if tuple(key) not in keys:
+          raise NotImplementedError("candidate ensemble %s drops %s (iteration %d) from the previous ensemble, but %s reads "
+                                    "its hidden layers" % (c.name, key[1], key[0], who))
 
   def train_iteration(self, batches: Iterator, steps: int, on_step=None) -> float:
     """Runs `steps` training steps; returns device seconds (CUDA events) of the phase.
@@ -304,11 +318,12 @@ class AdaNetSearch:
           if m.batch != self.batch:      # trained on a row slice: frozen replay needs full-minibatch buffers
             ws_, bs_ = m.numpy_params()
             new_members[k] = eng.DenseNet(m.name, m.dims, ws_, bs_, m.complexity, self.batch, self.device, t, m.shared,
-                                          m.image_shape)
+                                          m.image_shape, inputs=m.inputs, members=kept)
         mix_ws, bias = head.mixture_weight_tensors(), head.bias
       else:
         new_members = [eng.DenseNet(specs[b].name, specs[b].dims, specs[b].ws, specs[b].bs, specs[b].complexity,
-                                    self.batch, self.device, t, specs[b].shared, specs[b].image_shape)
+                                    self.batch, self.device, t, specs[b].shared, specs[b].image_shape,
+                                    inputs=getattr(specs[b], "inputs", None), members=kept)
                        for b in ec.builders]
         n_members = len(kept) + len(new_members)
         if matrix:

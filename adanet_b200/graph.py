@@ -189,6 +189,29 @@ def relu(x: Tensor) -> Tensor:
   return Tensor(x.shape, "relu", (x,))
 
 
+def concat(values: Sequence[Tensor], axis: int = -1) -> Tensor:
+  """tf.concat [TF] of rank-2 tensors [batch, width] on the last axis: what a builder uses to read the hidden layers
+  of previous-iteration subnetworks (adanet/core/estimator_test.py _DNNBuilder).  The engine lowers a dense layer over
+  it to one GEMM over the pieces (core/lowering.py); any other axis or rank raises NotImplementedError."""
+  values = list(values)
+  if not values or not all(isinstance(v, Tensor) for v in values):
+    raise ValueError("concat expects a non-empty list of Tensors, got %r" % (values,))
+  ranks = {len(v.shape) for v in values}
+  if len(ranks) != 1:
+    raise ValueError("concat of tensors of different ranks: %s" % ([v.shape for v in values],))
+  rank = ranks.pop()
+  if rank != 2:
+    raise NotImplementedError("concat is implemented for rank-2 tensors [batch, width] (got rank %d)" % rank)
+  if not -rank <= axis < rank:
+    raise ValueError("concat axis %d is out of range for rank-2 tensors" % axis)
+  if axis % rank != rank - 1:
+    raise NotImplementedError("concat is implemented on the last axis only (got axis=%d)" % axis)
+  batch = {v.shape[0] for v in values} - {None}
+  if len(batch) > 1:
+    raise ValueError("concat of tensors with different batch dimensions: %s" % ([v.shape for v in values],))
+  return Tensor((batch.pop() if batch else None, sum(int(v.shape[-1]) for v in values)), "concat", values)
+
+
 def dense(inputs: Tensor, units: int, activation=None, use_bias: bool = True, kernel_initializer=None,
           bias_initializer=None, name: Optional[str] = None) -> Tensor:
   """tf.layers.dense [TF]: kernel [in, units] (default glorot-uniform), bias zeros."""
