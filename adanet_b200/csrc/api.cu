@@ -207,6 +207,7 @@ static int check_fwd_op(const adn_fwd_op& op, int64_t batch, const char* what, p
   }
   if (ns > 0 && k_total > INT32_MAX) return fail(ADN_ERR_INVALID, "%s: total K too large", what);
   if ((op.yp == nullptr) == (op.y == nullptr)) return fail(ADN_ERR_INVALID, "%s: exactly one of yp / y", what);
+  if (op.yp && !pl::planes_aligned(op.yp)) return fail(ADN_ERR_INVALID, "%s: yp: plane buffers must be 256 B aligned", what);
   if (bad_shape(batch, op.in, op.out)) return fail(ADN_ERR_INVALID, "%s: bad shape", what);
   if (op.act != ADN_ACT_NONE && op.act != ADN_ACT_RELU) return fail(ADN_ERR_INVALID, "%s: bad act %d", what, op.act);
   if (op.dropout_rate != 0.f) {
@@ -225,6 +226,7 @@ static int check_bwd_op(const adn_bwd_op& p, int64_t batch, const char* what, pl
   if (!p.xp || !p.dzp || !p.workspace) return fail(ADN_ERR_INVALID, "%s: null pointer", what);
   if ((p.dxp || p.dx) && !p.wp) return fail(ADN_ERR_INVALID, "%s: wp required for dx", what);
   if (p.dxp && p.dx) return fail(ADN_ERR_INVALID, "%s: at most one of dxp / dx", what);
+  if (p.dxp && !pl::planes_aligned(p.dxp)) return fail(ADN_ERR_INVALID, "%s: dxp: plane buffers must be 256 B aligned", what);
   if (p.dx_colsum && !(p.dxp || p.dx)) return fail(ADN_ERR_INVALID, "%s: dx_colsum needs dx", what);
   if (bad_shape(batch, p.in, p.out)) return fail(ADN_ERR_INVALID, "%s: bad shape", what);
   if (p.dz_log2_scale < -60 || p.dz_log2_scale > 60) return fail(ADN_ERR_INVALID, "%s: bad dz_log2_scale", what);

@@ -46,9 +46,7 @@ __device__ __forceinline__ uint32_t sw128(int row, int k) {
 template <int N>
 __device__ __forceinline__ void mma_tf32(float (&d)[N / 2], uint32_t a_addr, uint32_t b_addr, uint32_t scale_d) {
   const uint64_t da = wg::desc_sw128(a_addr), db = wg::desc_sw128(b_addr);
-  if constexpr (N == 16) wg::mma_tf32_n16(d, da, db, scale_d);
-  else if constexpr (N == 48) wg::mma_tf32_n48(d, da, db, scale_d);
-  else if constexpr (N == 64) wg::mma_tf32_n64(d, da, db, scale_d);
+  if constexpr (N == 64) wg::mma_tf32_n64(d, da, db, scale_d);
   else wg::mma_tf32_n128(d, da, db, scale_d);
 }
 
@@ -226,223 +224,6 @@ conv_stem_tc_fwd_kernel(const float* __restrict__ images, const float* __restric
   }
 }
 
-// ---------------------------------------------------------------------------------------------------------------
-// Backward of the stem on the tensor cores: with G'[p][(pos, f)] = g[p][f] * [argmax(p, f) == pos] (the pooled-feature
-// gradient routed to its arg-max position) the kernel gradient of the expanded weights is
-//     dW'[(pos, f)][k] = sum_p G'[p][(pos, f)] * A[p][k]
-// -- a GEMM whose reduction runs over pooled pixels, so both operands are staged TRANSPOSED (K-major in the pooled
-// index): M side = G'^T [4F = 64 rows][64 px], N side = A^T [K rows][64 px], 3xTF32, 24 wgmma (M64 N=K K8) per tile
-// of 64 pooled pixels.  A warpgroup's 128 threads split the building of a tile: threads 0-63 build A^T from the
-// staged image, threads 64-127 fetch g / arg-max from global memory and build G'^T; all 128 issue the MMAs.
-// Two-level accumulation: the MMAs sum one tile, which is then added (RN) into a register accumulator; at the end
-// dK[ky,kx,c,f] = sum_pos dW'[(pos,f)][(ky+dy, kx+dx, c)] is folded in fixed order and written as this CTA's partial
-// (same format as the SIMT backward, reduced by conv_stem_reduce_kernel).
-template <int CIN, int F>
-__global__ void __launch_bounds__(THREADS, 1)
-conv_stem_tc_bwd_kernel(const float* __restrict__ images, const uint32_t* __restrict__ argmax,
-                        const float* __restrict__ dpooled, float* __restrict__ partials, int64_t B, int H, int W) {
-  constexpr int K = 16 * CIN;              // patch size = GEMM N
-  static_assert(4 * F == 64, "(pos, f) rows are the 64 rows of one wgmma");
-  constexpr int PXT = 64;                  // pooled pixels per tile = GEMM K
-  constexpr int GB = 2 * TILE_BYTES;       // one plane of G'^T: 2 k-blocks of [128 rows][32 px] (rows 64.. unused)
-  constexpr int AB = 2 * K * 128;          // one plane of A^T : 2 k-blocks of [K rows][32 px]
-  constexpr int WGB = 2 * GB + 2 * AB;     // bytes per warpgroup
-  constexpr int K9 = 9 * CIN;
-  extern __shared__ __align__(16) uint8_t smem_raw[];
-  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const int pimg = (H + 2) * (W + 2) * CIN;
-  float* s_img0 = reinterpret_cast<float*>(base + 2 * WGB);
-
-  const int tid = threadIdx.x, lane = tid & 31;
-  const int wg = tid >> 7, r = tid & 127, wq = (tid >> 5) & 3;
-  const int gid = lane >> 2, tq = lane & 3;
-  const int half = r >> 6, q = r & 63;     // half 0: A^T builder, half 1: G'^T builder
-  uint8_t* g_hi = base + wg * WGB;
-  uint8_t* g_lo = g_hi + GB;
-  uint8_t* at_hi = g_lo + GB;
-  uint8_t* at_lo = at_hi + AB;
-  for (int i = tid; i < (2 * WGB) / 16; i += THREADS) reinterpret_cast<float4*>(base)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-  for (int i = tid; i < 2 * pimg; i += THREADS) s_img0[i] = 0.f;
-  __syncthreads();
-  const uint32_t g_addr = smem_u32(g_hi), at_addr = smem_u32(at_hi);
-
-  const int PH = H / 2, PW = W / 2, P = PH * PW;
-  const int tiles = (P + PXT - 1) / PXT;
-  const int prow = (W + 2) * CIN;
-  const int64_t img_elems = (int64_t)H * W * CIN;
-  const int64_t cols = (int64_t)P * F;
-  float acc[K / 2];                        // dW' fragment: rows 16 wq + gid (+8), columns 8 j + 2 tq (+1)
-#pragma unroll
-  for (int k = 0; k < K / 2; ++k) acc[k] = 0.f;
-  float accb[F];                           // G builders: sum of g over their pooled pixels, per filter
-#pragma unroll
-  for (int f = 0; f < F; ++f) accb[f] = 0.f;
-
-  int64_t b = blockIdx.x;
-  int buf = 0;
-  if (b < B) stage_image<CIN>(s_img0, images + b * img_elems, H, W, tid);
-  cp_async_commit();
-  for (; b < B; b += gridDim.x, buf ^= 1) {
-    const int64_t nb = b + gridDim.x;
-    if (nb < B) stage_image<CIN>(s_img0 + (buf ^ 1) * pimg, images + nb * img_elems, H, W, tid);
-    cp_async_commit();
-    cp_async_wait<1>();
-    __syncthreads();
-    const float* s_img = s_img0 + buf * pimg;
-    for (int tile = wg; tile < tiles; tile += 2) {
-      const int p = tile * PXT + q;
-      const bool valid = p < P;
-      const uint32_t kblk = (uint32_t)(q >> 5);      // which 32-pixel k-block this pooled pixel falls in
-      const int col = q & 31;
-      if (half == 0) {
-        // ---- A^T: column `q` of every row k (the 4x4xCIN patch of pooled pixel p) ----
-        const int py = valid ? p / PW : 0, px = valid ? p - py * PW : 0;
-        const float* patch = s_img + (2 * py) * prow + (2 * px) * CIN;
-#pragma unroll
-        for (int c4 = 0; c4 < K / 4; ++c4) {
-          const int i = (CIN == 3) ? c4 / 3 : c4;
-          const int o = (CIN == 3) ? (c4 % 3) * 4 : 0;
-          float2 v0 = *reinterpret_cast<const float2*>(patch + i * prow + o);
-          float2 v1 = *reinterpret_cast<const float2*>(patch + i * prow + o + 2);
-          if (!valid) { v0 = make_float2(0.f, 0.f); v1 = v0; }
-          const float v[4] = {v0.x, v0.y, v1.x, v1.y};
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const int k = c4 * 4 + e;
-            float h, l;
-            pl::split_tf32(v[e], h, l);
-            const uint32_t off = kblk * (uint32_t)(K * 128) + sw128(k, col);
-            *reinterpret_cast<float*>(at_hi + off) = h;
-            *reinterpret_cast<float*>(at_lo + off) = l;
-          }
-        }
-      } else {
-        // ---- G'^T: column `q` of rows (pos, f): g at the arg-max position, zero at the other three ----
-#pragma unroll
-        for (int f0 = 0; f0 < F; f0 += 16) {
-          float g[16];
-          uint32_t aw = 0u;
-          if (valid) {
-            const float4* src = reinterpret_cast<const float4*>(dpooled + b * cols + (int64_t)p * F + f0);
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const float4 t = __ldg(src + e);
-              g[4 * e] = t.x; g[4 * e + 1] = t.y; g[4 * e + 2] = t.z; g[4 * e + 3] = t.w;
-            }
-            aw = __ldg(argmax + b * (cols / 16) + ((int64_t)p * F + f0) / 16);
-          } else {
-#pragma unroll
-            for (int e = 0; e < 16; ++e) g[e] = 0.f;
-          }
-#pragma unroll
-          for (int e = 0; e < 16; ++e) {
-            const uint32_t pos = (aw >> (2 * e)) & 3u;
-            float h, l;
-            pl::split_tf32(g[e], h, l);
-            accb[f0 + e] += g[e];
-#pragma unroll
-            for (int s = 0; s < 4; ++s) {
-              const uint32_t off = kblk * (uint32_t)TILE_BYTES + sw128(s * F + f0 + e, col);
-              *reinterpret_cast<float*>(g_hi + off) = (pos == (uint32_t)s) ? h : 0.f;
-              *reinterpret_cast<float*>(g_lo + off) = (pos == (uint32_t)s) ? l : 0.f;
-            }
-          }
-        }
-      }
-      fence_async_smem();
-      wg_barrier(wg);
-      float d[K / 2];
-#pragma unroll
-      for (int k = 0; k < K / 2; ++k) d[k] = 0.f;
-      wg::fence_regs(d);
-      wg::fence();
-#pragma unroll
-      for (int prod = 0; prod < 3; ++prod) {       // g_hi a_hi, g_lo a_hi, g_hi a_lo
-        const uint32_t gg = g_addr + (prod == 1 ? GB : 0);
-        const uint32_t aa = at_addr + (prod == 2 ? AB : 0);
-#pragma unroll
-        for (int ks = 0; ks < PXT / 8; ++ks)
-          mma_tf32<K>(d, gg + (ks >> 2) * TILE_BYTES + (ks & 3) * 32, aa + (ks >> 2) * (K * 128) + (ks & 3) * 32,
-                      (prod == 0 && ks == 0) ? 0u : 1u);
-      }
-      wg::commit();
-      wg::wait<0>();
-      wg::fence_regs(d);
-#pragma unroll
-      for (int k = 0; k < K / 2; ++k) acc[k] += d[k];
-      wg_barrier(wg);                      // every warp's MMAs are done before the operands are rebuilt
-    }
-    __syncthreads();
-  }
-  // ---- fold: dump dW' and the bias sums to shared memory (the operand tiles are free now), then fixed-order sums ----
-  __syncthreads();
-  float* s_d = reinterpret_cast<float*>(base);                  // [2 wg][64 rows][K]
-  float* s_db = s_d + 2 * 64 * K;                               // [2 wg][64 px][F]
-#pragma unroll
-  for (int j = 0; j < K / 8; ++j)
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      const int row = 16 * wq + gid + 8 * (e >> 1), k = 8 * j + 2 * tq + (e & 1);
-      s_d[(wg * 64 + row) * K + k] = acc[4 * j + e];
-    }
-  if (half == 1) {
-#pragma unroll
-    for (int f = 0; f < F; ++f) s_db[(wg * 64 + q) * F + f] = accb[f];
-  }
-  __syncthreads();
-  float* mine = partials + (size_t)blockIdx.x * (K9 * F + F);
-  for (int t = tid; t < K9 * F; t += THREADS) {
-    const int f = t % F, kc = t / F;                            // kc = (ky*3 + kx)*CIN + c
-    const int c = kc % CIN, kyx = kc / CIN, ky = kyx / 3, kx = kyx - ky * 3;
-    float sum = 0.f;
-    for (int w2 = 0; w2 < 2; ++w2)
-      for (int pos = 0; pos < 4; ++pos) {
-        const int n = pos * F + f;
-        if (n < 64) {
-          const int k = ((ky + (pos >> 1)) * 4 + (kx + (pos & 1))) * CIN + c;
-          sum += s_d[(w2 * 64 + n) * K + k];
-        }
-      }
-    mine[t] = sum;
-  }
-  for (int f = tid; f < F; f += THREADS) {
-    float sum = 0.f;
-    for (int i = 0; i < 2 * 64; ++i) sum += s_db[i * F + f];
-    mine[K9 * F + f] = sum;
-  }
-}
-
-template <int CIN, int F>
-static size_t bwd_smem_bytes(int h, int w) {
-  constexpr int K = 16 * CIN;
-  return 1024 + (size_t)2 * (2 * 2 * TILE_BYTES + 2 * 2 * K * 128) + (size_t)2 * (h + 2) * (w + 2) * CIN * 4;
-}
-
-bool bwd_supported(int h, int w, int cin, int f) {
-  if (f != 16) return false;               // (pos, f) rows are the 64 rows of one wgmma
-  const size_t smem = cin == 3 ? bwd_smem_bytes<3, 16>(h, w) : bwd_smem_bytes<1, 16>(h, w);
-  return smem <= 227 * 1024;
-}
-
-// writes `*n_partials` per-CTA partials [9*cin*f + f] into `partials`
-int bwd(const float* images, const uint32_t* argmax, const float* dpooled, float* partials, int* n_partials, int64_t batch,
-        int h, int w, int cin, int f, cudaStream_t st) {
-  const int64_t cap = sm_count();
-  const int grid = (int)(batch < cap ? batch : cap);
-  *n_partials = grid;
-  if (cin == 3) {
-    const size_t smem = bwd_smem_bytes<3, 16>(h, w);
-    auto kern = conv_stem_tc_bwd_kernel<3, 16>;
-    kern<<<grid, THREADS, smem, st>>>(images, argmax, dpooled, partials, batch, h, w);
-  } else {
-    const size_t smem = bwd_smem_bytes<1, 16>(h, w);
-    auto kern = conv_stem_tc_bwd_kernel<1, 16>;
-    kern<<<grid, THREADS, smem, st>>>(images, argmax, dpooled, partials, batch, h, w);
-  }
-  ADN_CHECK_LAUNCH("conv_stem_tc_bwd");
-  return ADN_OK;
-}
-
 template <int CIN, int F>
 static size_t smem_bytes(int h, int w) {
   constexpr int K = 16 * CIN, KB = (K + 31) / 32, N = 4 * F;
@@ -467,7 +248,6 @@ int init() {
 #define ADN_CONVTC_ATTR(K) ADN_CUDA(cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024))
   ADN_CONVTC_ATTR((conv_stem_tc_fwd_kernel<1, 16>)); ADN_CONVTC_ATTR((conv_stem_tc_fwd_kernel<3, 16>));
   ADN_CONVTC_ATTR((conv_stem_tc_fwd_kernel<1, 32>)); ADN_CONVTC_ATTR((conv_stem_tc_fwd_kernel<3, 32>));
-  ADN_CONVTC_ATTR((conv_stem_tc_bwd_kernel<1, 16>)); ADN_CONVTC_ATTR((conv_stem_tc_bwd_kernel<3, 16>));
 #undef ADN_CONVTC_ATTR
   return ADN_OK;
 }

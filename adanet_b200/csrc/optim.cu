@@ -186,7 +186,6 @@ struct StepPtrs {
 __global__ void step_increment_group_kernel(const __grid_constant__ StepPtrs s) {
   if ((int)threadIdx.x < s.n) *s.p[threadIdx.x] += 1;
 }
-__global__ void step_increment_kernel(int64_t* step) { *step += 1; }
 
 }  // namespace adn
 

@@ -29,7 +29,7 @@
 // Kernel (pl_gemm_kernel): persistent, grouped, 512 threads = TMA producer warpgroup + 2 consumer warpgroups of 64
 // rows of a 128 x 64 tile + an epilogue warpgroup.  The consumers write each finished tile's accumulators into one of
 // two swizzled 32 KiB staging tiles and go on with the next tile's mainloop; the epilogue warpgroup reads the tile
-// back row-per-lane and runs bias/ReLU/dropout, masks, column sums and the stores (plane tiles leave by TMA).
+// back row-per-lane and runs bias/ReLU/dropout, masks, column sums and the stores (fp16 plane tiles leave by TMA).
 // The epilogue is the pace-setter of the thin-K waves, so its per-tile chain is kept short: the accumulators stay in
 // registers, the global words a tile needs (ReLU mask, dropout step) are loaded one work item ahead, and each warp
 // has a hi and a lo' store slab, so a slice never waits for a TMA store it has just issued.
@@ -102,18 +102,16 @@ struct GemmParams {
   int M, N;
   int tiles_m, tiles_n, splits;
   int tiles;             // tiles_m * tiles_n
-  float inv_tiles, inv_tiles_n, inv_tiles_m;   // reciprocals for the division-free item decode (counts stay far below 2^21)
+  float inv_tiles, inv_tiles_n;   // reciprocals for the division-free item decode (counts stay far below 2^21)
   int total_kb;          // k-blocks over the whole K
   int kb_per_split;
   int a_mn, b_mn;        // operand majorness (0 = K-major box, 1 = MN-major box)
   int out_planes;        // 1: result written as split planes (out / out_lo / out_bits), 0: dense fp32
-  int m_fastest;         // work-item order: 1 = row blocks fastest (write locality), 0 = column blocks fastest (A reuse in L2)
   // output: dense row-major (ldc) / split-K partial [split][M][N], or planes
   void* out;             // dense base | hi plane base
-  void* out_lo;          // lo plane base (OUT_PLANES)
+  void* out_lo;          // lo plane base (out_planes)
   int ldc;
   int out_nb32;          // planes: 32-column blocks of the (padded) output tensor
-  int out_tma;           // planes (fp16): the tile is written through shared memory with TMA stores (Problem::o_hi / o_lo)
   const float* bias;     // EPI_BIAS_ACT (nullable)
   int act;
   uint32_t* out_bits;    // planes + EPI_BIAS_ACT: sign bits of the output
@@ -202,15 +200,9 @@ __device__ __forceinline__ Item decode_item(const GemmParams& g, int item) {
   Item it;
   it.split = (g.splits == 1) ? 0 : fast_div(item, g.inv_tiles);
   const int t = item - it.split * g.tiles;
-  if (g.m_fastest) {            // consecutive items = consecutive row blocks of the same column block
-    const int tn = fast_div(t, g.inv_tiles_m);
-    it.n0 = tn * BN;
-    it.m0 = (t - tn * g.tiles_m) * BM;
-  } else {
-    const int tm = (g.tiles_n == 1) ? t : fast_div(t, g.inv_tiles_n);
-    it.m0 = tm * BM;
-    it.n0 = (t - tm * g.tiles_n) * BN;
-  }
+  const int tm = (g.tiles_n == 1) ? t : fast_div(t, g.inv_tiles_n);
+  it.m0 = tm * BM;
+  it.n0 = (t - tm * g.tiles_n) * BN;
   it.kb0 = it.split * g.kb_per_split;
   it.nkb = min(g.total_kb, it.kb0 + g.kb_per_split) - it.kb0;
   return it;
@@ -220,59 +212,37 @@ __device__ __forceinline__ uint32_t pack_h2(__half a, __half b) {
   return (uint32_t)__half_as_ushort(a) | ((uint32_t)__half_as_ushort(b) << 16);
 }
 
-// One 32-row x 32-column slice of a tile: lane = row holds its 32 accumulators a[0..31] (columns
-// cbase..cbase+31).  Applies bias/ReLU (+ sign bits) or the sign-bit ReLU mask in the register layout,
-// transposes through `stage` (16 B chunks XOR-swizzled by row: conflict-free both ways) and writes with
-// lane = 4-column group of 8 rows, so every global access covers whole 32 B sectors.
 __device__ __forceinline__ void st_global_v8(void* p, const uint32_t (&w)[8]) {   // 32 B as two 16 B stores
   uint4* q = reinterpret_cast<uint4*>(p);
   q[0] = make_uint4(w[0], w[1], w[2], w[3]);
   q[1] = make_uint4(w[4], w[5], w[6], w[7]);
 }
 
-// split 32 values of one row into the two planes and write them with 32 B per store pair (TF32 planes, and fp16
-// planes under ADN_PL_TMA_STORE=0; the default fp16 path is store_slice_tma_hi / _lo below)
-template <int FMT>
-__device__ __forceinline__ void store_row32_planes(const GemmParams& g, const float* a, int my_row, int cbase) {
-  constexpr int BK = Fmt<FMT>::BK;
+// split 32 values of one row into the two TF32 planes and write them with 32 B per store pair (TF32 planes have no
+// TMA store path: the fp16 planes leave through store_slice_tma below)
+__device__ __forceinline__ void store_row32_tf32(const GemmParams& g, const float* a, int my_row, int cbase) {
+  constexpr int BK = Fmt<FMT_TF32>::BK;
   const size_t poff = ((size_t)(cbase / BK) * g.M + my_row) * BK + (cbase % BK);
-  if (FMT == FMT_F16) {
-    uint32_t hw[16], lw[16];
+  uint32_t hw[32], lw[32];
 #pragma unroll
-    for (int q = 0; q < 16; ++q) {
-      const __half2 h2 = __floats2half2_rn(a[2 * q], a[2 * q + 1]);
-      const float2 hf = __half22float2(h2);
-      const __half2 l2 = __floats2half2_rn((a[2 * q] - hf.x) * 2048.0f, (a[2 * q + 1] - hf.y) * 2048.0f);
-      hw[q] = *reinterpret_cast<const uint32_t*>(&h2);
-      lw[q] = *reinterpret_cast<const uint32_t*>(&l2);
-    }
-    __half* hp = reinterpret_cast<__half*>(g.out) + poff;
-    __half* lp = reinterpret_cast<__half*>(g.out_lo) + poff;
-    st_global_v8(hp, reinterpret_cast<const uint32_t(&)[8]>(hw[0]));
-    st_global_v8(hp + 16, reinterpret_cast<const uint32_t(&)[8]>(hw[8]));
-    st_global_v8(lp, reinterpret_cast<const uint32_t(&)[8]>(lw[0]));
-    st_global_v8(lp + 16, reinterpret_cast<const uint32_t(&)[8]>(lw[8]));
-  } else {
-    uint32_t hw[32], lw[32];
+  for (int j = 0; j < 32; ++j) {
+    float h, l;
+    split_tf32(a[j], h, l);
+    hw[j] = __float_as_uint(h);
+    lw[j] = __float_as_uint(l);
+  }
+  float* hp = reinterpret_cast<float*>(g.out) + poff;
+  float* lp = reinterpret_cast<float*>(g.out_lo) + poff;
 #pragma unroll
-    for (int j = 0; j < 32; ++j) {
-      float h, l;
-      split_tf32(a[j], h, l);
-      hw[j] = __float_as_uint(h);
-      lw[j] = __float_as_uint(l);
-    }
-    float* hp = reinterpret_cast<float*>(g.out) + poff;
-    float* lp = reinterpret_cast<float*>(g.out_lo) + poff;
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      st_global_v8(hp + 8 * q, reinterpret_cast<const uint32_t(&)[8]>(hw[8 * q]));
-      st_global_v8(lp + 8 * q, reinterpret_cast<const uint32_t(&)[8]>(lw[8 * q]));
-    }
+  for (int q = 0; q < 4; ++q) {
+    st_global_v8(hp + 8 * q, reinterpret_cast<const uint32_t(&)[8]>(hw[8 * q]));
+    st_global_v8(lp + 8 * q, reinterpret_cast<const uint32_t(&)[8]>(lw[8 * q]));
   }
 }
 
-// The same slice through shared memory and TMA (fp16 planes).  With the direct stores above every lane of a store
-// instruction touches a different 128 B line, which the load/store unit serialises into 16 B wavefronts.  Here a lane writes its row's 64 B of one plane into the warp's 2 KB staging
+// The same slice of fp16 planes, through shared memory and TMA.  With direct stores from the row-owning lanes every
+// lane of a store instruction would touch a different 128 B line, which the load/store unit serialises into 16 B
+// wavefronts.  Here a lane writes its row's 64 B of one plane into the warp's 2 KB staging
 // slab (16 B chunks XOR-swizzled the way CU_TENSOR_MAP_SWIZZLE_64B expects: chunk ^= (row >> 1) & 3, conflict-free)
 // and one lane hands the [32 rows][32 columns] box to the TMA unit.  Rows past M are clipped by the tensor map.
 // The hi and lo' planes have a slab each, and every slice commits its hi store and then its lo' store, so before a
@@ -315,7 +285,7 @@ __device__ __forceinline__ void store_slice_tma(const CUtensorMap* o_hi, const C
 // Forward epilogue with planes out, WITHOUT a register transpose: lane = row keeps its 32 accumulators (bias already
 // added by the caller), applies ReLU / dropout, forms the sign-bit word, splits pairs of values with packed conversions
 // and hands its 32 columns of each plane to the slab + TMA store path (fp16) or writes them with direct 16 B stores
-// (TF32: 128 B per plane).  ~10 instructions per element against ~29 of the staged path.
+// (TF32: 128 B per plane).
 template <int FMT>
 __device__ __forceinline__ void emit_slice_fwd_planes(const GemmParams& g, float* a, uint32_t drop_step, int lane, int mrow0,
                                                       int cbase, const CUtensorMap* o_hi, const CUtensorMap* o_lo,
@@ -345,8 +315,8 @@ __device__ __forceinline__ void emit_slice_fwd_planes(const GemmParams& g, float
     for (int j = 0; j < 32; ++j)
       if (!((cmask >> j) & 1u)) a[j] = 0.f;
   }
-  if (FMT == FMT_F16 && g.out_tma) store_slice_tma(o_hi, o_lo, slab_hi, slab_lo, a, lane, mrow0, cbase);
-  else if (my_row < g.M) store_row32_planes<FMT>(g, a, my_row, cbase);
+  if (FMT == FMT_F16) store_slice_tma(o_hi, o_lo, slab_hi, slab_lo, a, lane, mrow0, cbase);
+  else if (my_row < g.M) store_row32_tf32(g, a, my_row, cbase);
   uint32_t bits = 0u;
 #pragma unroll
   for (int j = 0; j < 32; ++j) bits |= (a[j] > 0.f) ? (1u << j) : 0u;
@@ -368,10 +338,10 @@ __device__ __forceinline__ void colsum_round(float* a, int lane) {
 }
 
 // dX epilogue with planes out, without a register transpose: sign-bit ReLU mask, plane stores as in the forward
-// epilogue (slab + TMA, or direct stores from the row-owning lane), and the per-32-row column sums (the bias
-// gradient of the layer below) by a butterfly over the warp: at distance w a lane keeps the half of its columns selected by bit w of its lane id and receives the partner's
-// partial sums for them, so after five rounds lane l holds the sum of column l over the 32 rows (31 shuffles and
-// adds per lane, fixed order).
+// epilogue (slab + TMA for fp16, direct stores from the row-owning lane for TF32), and the per-32-row column sums
+// (the bias gradient of the layer below) by a butterfly over the warp: at distance w a lane keeps the half of its
+// columns selected by bit w of its lane id and receives the partner's partial sums for them, so after five rounds
+// lane l holds the sum of column l over the 32 rows (31 shuffles and adds per lane, fixed order).
 template <int FMT>
 __device__ __forceinline__ void emit_slice_mask_planes(const GemmParams& g, float* a, uint32_t mwq, int lane, int mrow0, int cbase,
                                                        const CUtensorMap* o_hi, const CUtensorMap* o_lo, uint32_t slab_hi,
@@ -390,8 +360,8 @@ __device__ __forceinline__ void emit_slice_mask_planes(const GemmParams& g, floa
     for (int j = 0; j < 32; ++j)
       if (!((keep >> j) & 1u)) a[j] = 0.f;
   }
-  if (FMT == FMT_F16 && g.out_tma) store_slice_tma(o_hi, o_lo, slab_hi, slab_lo, a, lane, mrow0, cbase);
-  else if (my_row < g.M) store_row32_planes<FMT>(g, a, my_row, cbase);
+  if (FMT == FMT_F16) store_slice_tma(o_hi, o_lo, slab_hi, slab_lo, a, lane, mrow0, cbase);
+  else if (my_row < g.M) store_row32_tf32(g, a, my_row, cbase);
   if (g.colsum_part) {
     colsum_round<16>(a, lane);
     colsum_round<8>(a, lane);
@@ -403,18 +373,23 @@ __device__ __forceinline__ void emit_slice_mask_planes(const GemmParams& g, floa
   }
 }
 
+// One 32-row x 32-column slice of a tile: lane = row holds its 32 accumulators a[0..31] (columns cbase..cbase+31,
+// the bias already in them).  Plane outputs go to the two functions above.  Everything else is a dense fp32 output
+// (the logits y, the conv stem's dense dX, the dW split-K partials): ReLU, or the scale and the sign-bit ReLU mask,
+// are applied in the register layout, then the slice is transposed through `stage` (16 B chunks XOR-swizzled by row:
+// conflict-free both ways) and written with lane = 4-column group of 8 rows, so every global access covers whole
+// 32 B sectors.
 template <int FMT, int EPI>
-__device__ __forceinline__ void emit_slice(const GemmParams& g, const bool OUT_PLANES, float* a, uint32_t mwq, float* stage,
+__device__ __forceinline__ void emit_slice(const GemmParams& g, const bool out_planes, float* a, uint32_t mwq, float* stage,
                                            int lane, int mrow0, int cbase, int rows_ok, float* dense, bool dense_vec,
-                                           const bool bias_in_acc = false, const CUtensorMap* o_hi = nullptr,
-                                           const CUtensorMap* o_lo = nullptr, uint32_t drop_step = 0u) {
+                                           const CUtensorMap* o_hi, const CUtensorMap* o_lo, uint32_t drop_step) {
   // `stage` is the warp's hi slab; its lo' slab follows it
-  if (EPI == EPI_BIAS_ACT && OUT_PLANES && bias_in_acc) {
+  if (EPI == EPI_BIAS_ACT && out_planes) {
     emit_slice_fwd_planes<FMT>(g, a, drop_step, lane, mrow0, cbase, o_hi, o_lo, smem_u32(stage),
                                smem_u32(stage + EPI_STAGE_FLOATS));
     return;
   }
-  if (EPI == EPI_MASK && OUT_PLANES && bias_in_acc) {      // (the single-CTA kernel's direct path; out_mul is 1 for planes)
+  if (EPI == EPI_MASK && out_planes) {
     emit_slice_mask_planes<FMT>(g, a, mwq, lane, mrow0, cbase, o_hi, o_lo, smem_u32(stage), smem_u32(stage + EPI_STAGE_FLOATS));
     return;
   }
@@ -423,41 +398,11 @@ __device__ __forceinline__ void emit_slice(const GemmParams& g, const bool OUT_P
   constexpr int RPI = 32 / CH;             // rows covered by one transposed instruction (8)
   const int cc = lane % CH;                // 16 B chunk (4 columns) this lane owns after the transpose
   const int rsub = lane / CH;
-  const int my_row = mrow0 + lane;
-  const int kbo = cbase >> 5;              // 32-column block of the output
-  const bool live = (OUT_PLANES ? (kbo < g.out_nb32) : (cbase < g.N)) && rows_ok > 0;   // warp-uniform
-  // valid columns of this slice as a bit mask (warp-uniform); all ones for interior tiles
-  const uint32_t cmask = (cbase + 32 <= g.N) ? 0xffffffffu : ((cbase < g.N) ? ((1u << (g.N - cbase)) - 1u) : 0u);
+  const bool live = cbase < g.N && rows_ok > 0;   // warp-uniform
   if (EPI == EPI_BIAS_ACT) {
-    if (g.bias && !bias_in_acc) {
-      if (cmask == 0xffffffffu && (reinterpret_cast<uintptr_t>(g.bias) & 15) == 0) {
-#pragma unroll
-        for (int jj = 0; jj < 8; ++jj) {
-          const float4 bv = __ldg(reinterpret_cast<const float4*>(g.bias + cbase) + jj);   // warp-uniform address
-          a[4 * jj + 0] += bv.x; a[4 * jj + 1] += bv.y;
-          a[4 * jj + 2] += bv.z; a[4 * jj + 3] += bv.w;
-        }
-      } else {
-#pragma unroll
-        for (int j = 0; j < 32; ++j)
-          if ((cmask >> j) & 1u) a[j] += __ldg(g.bias + cbase + j);
-      }
-    }
     if (g.act == ADN_ACT_RELU) {
 #pragma unroll
       for (int j = 0; j < 32; ++j) a[j] = fmaxf(a[j], 0.f);
-    }
-    if (OUT_PLANES) {
-      uint32_t bits = 0u;
-#pragma unroll
-      for (int j = 0; j < 32; ++j) bits |= (a[j] > 0.f) ? (1u << j) : 0u;
-      bits &= cmask;
-      if (live && my_row < g.M) g.out_bits[(size_t)kbo * g.M + my_row] = bits;
-    }
-    if (cmask != 0xffffffffu) {       // K padding of the next GEMM must be exact zeros
-#pragma unroll
-      for (int j = 0; j < 32; ++j)
-        if (!((cmask >> j) & 1u)) a[j] = 0.f;
     }
   } else {
     if (g.out_mul != 1.0f) {
@@ -465,6 +410,8 @@ __device__ __forceinline__ void emit_slice(const GemmParams& g, const bool OUT_P
       for (int j = 0; j < 32; ++j) a[j] *= g.out_mul;
     }
     if (EPI == EPI_MASK) {
+      // valid columns of this slice as a bit mask (warp-uniform); all ones for interior tiles
+      const uint32_t cmask = (cbase + 32 <= g.N) ? 0xffffffffu : ((cbase < g.N) ? ((1u << (g.N - cbase)) - 1u) : 0u);
       const uint32_t keep = mwq & cmask;
       if (keep != 0xffffffffu) {
 #pragma unroll
@@ -490,9 +437,6 @@ __device__ __forceinline__ void emit_slice(const GemmParams& g, const bool OUT_P
       const int c4 = h * SW + cc * 4;       // column offset inside the 32-column slice
       const int col = cbase + c4;
       cs[0] = cs[1] = cs[2] = cs[3] = 0.f;
-      // plane element offset of (row mrow0 + rsub, column col): k-block-major, BK columns per k-block row
-      constexpr int BK = Fmt<FMT>::BK;
-      const size_t poff = OUT_PLANES ? ((size_t)(col / BK) * g.M + mrow0 + rsub) * BK + (col % BK) : 0;
 #pragma unroll
       for (int i = 0; i < 32 / RPI; ++i) {
         const int r = rsub + RPI * i;
@@ -504,33 +448,13 @@ __device__ __forceinline__ void emit_slice(const GemmParams& g, const bool OUT_P
           for (int k = 0; k < 4; ++k) cs[k] += rv ? v[k] : 0.f;
         }
         if (rv) {
-          if (OUT_PLANES) {
-            if (FMT == FMT_F16) {
-              __half hh[4], ll[4];
-#pragma unroll
-              for (int k = 0; k < 4; ++k) split_f16(v[k], hh[k], ll[k]);
-              __half* hp = reinterpret_cast<__half*>(g.out) + poff + (size_t)i * RPI * BK;
-              __half* lp = reinterpret_cast<__half*>(g.out_lo) + poff + (size_t)i * RPI * BK;
-              *reinterpret_cast<uint2*>(hp) = make_uint2(pack_h2(hh[0], hh[1]), pack_h2(hh[2], hh[3]));
-              *reinterpret_cast<uint2*>(lp) = make_uint2(pack_h2(ll[0], ll[1]), pack_h2(ll[2], ll[3]));
-            } else {
-              float hh[4], ll[4];
-#pragma unroll
-              for (int k = 0; k < 4; ++k) split_tf32(v[k], hh[k], ll[k]);
-              float* hp = reinterpret_cast<float*>(g.out) + poff + (size_t)i * RPI * BK;
-              float* lp = reinterpret_cast<float*>(g.out_lo) + poff + (size_t)i * RPI * BK;
-              *reinterpret_cast<float4*>(hp) = make_float4(hh[0], hh[1], hh[2], hh[3]);
-              *reinterpret_cast<float4*>(lp) = make_float4(ll[0], ll[1], ll[2], ll[3]);
-            }
+          float* op = dense + (size_t)(mrow0 + r) * g.ldc + col;
+          if (dense_vec && col + 3 < g.N) {
+            *reinterpret_cast<float4*>(op) = make_float4(v[0], v[1], v[2], v[3]);
           } else {
-            float* op = dense + (size_t)(mrow0 + r) * g.ldc + col;
-            if (dense_vec && col + 3 < g.N) {
-              *reinterpret_cast<float4*>(op) = make_float4(v[0], v[1], v[2], v[3]);
-            } else {
 #pragma unroll
-              for (int k = 0; k < 4; ++k)
-                if (col + k < g.N) op[k] = v[k];
-            }
+            for (int k = 0; k < 4; ++k)
+              if (col + k < g.N) op[k] = v[k];
           }
         }
       }
@@ -567,7 +491,7 @@ static constexpr int MAX_GROUP = 8;
 
 struct alignas(64) Problem {
   CUtensorMap a_hi, a_lo, b_hi, b_lo;
-  CUtensorMap o_hi, o_lo;   // output planes as [32 rows][32 columns] store boxes (GemmParams::out_tma)
+  CUtensorMap o_hi, o_lo;   // fp16 output planes as [32 rows][32 columns] store boxes
   GemmParams g;
   int item0;             // first work item of this problem
   int pad_[3];
@@ -866,8 +790,8 @@ __device__ __forceinline__ void pl_gemm_body(const G& grp) {
           if (lane == 0) bulk_wait_read0();
           __syncwarp();
         }
-        emit_slice<FMT, EPI>(g, out_planes, acc, mw, stage, lane, mrow0, ncol0, rows_ok, dense, dense_vec, true,
-                             &grp.p[e.p].o_hi, &grp.p[e.p].o_lo, e.drop_step);
+        emit_slice<FMT, EPI>(g, out_planes, acc, mw, stage, lane, mrow0, ncol0, rows_ok, dense, dense_vec, &grp.p[e.p].o_hi,
+                             &grp.p[e.p].o_lo, e.drop_step);
       }
     }
     if (FMT == FMT_F16 && lane == 0) bulk_wait0();    // stores complete before the CTA (and its shared memory) goes away
@@ -1202,11 +1126,6 @@ static int make_store_map(CUtensorMap* map, const void* plane, int64_t rows, int
   g_maps.emplace(key, *map);
   return ADN_OK;
 }
-static int store_mode() {      // ADN_PL_TMA_STORE=0: direct global stores instead (A/B switch)
-  static const int env = getenv("ADN_PL_TMA_STORE") ? atoi(getenv("ADN_PL_TMA_STORE")) : 1;
-  return env;
-}
-
 // one GEMM of a group: operands + epilogue description (tiles / item numbering are filled at launch)
 struct GemmDesc {
   Operand a, b;
@@ -1225,16 +1144,6 @@ static int encode_maps(int fmt, const GemmDesc& d, CUtensorMap* a_hi, CUtensorMa
   if ((rc = make_map(fmt, b_hi, d.b.hi, d.b.rows, d.b.nkb, d.b.mn_major, BN))) return rc;
   if ((rc = make_map(fmt, b_lo, d.b.lo, d.b.rows, d.b.nkb, d.b.mn_major, BN))) return rc;
   return ADN_OK;
-}
-
-// Work-item order of one problem.  Column blocks fastest lets the CTAs that run together share the A tile through
-// L2 (A is the big operand of the long-K layers); row blocks fastest makes them write adjacent 16 KB runs of the
-// same output k-block slab.  ADN_PL_MFAST: -1 heuristic (default), 0 / 1 force.
-static int item_order_m_fastest(const GemmParams& g) {
-  static const int env = getenv("ADN_PL_MFAST") ? atoi(getenv("ADN_PL_MFAST")) : -1;
-  if (env >= 0) return env;
-  (void)g;
-  return 0;
 }
 
 template <int FMT, int EPI>
@@ -1279,12 +1188,10 @@ static int build_groups(int fmt, const GemmDesc* d, int n, std::vector<G>& out, 
           if (kb != src.g.total_kb) return fail(ADN_ERR_INVALID, "%s: k-blocks of the pieces do not add up", what);
         }
         pr.g = src.g;
-        pr.g.out_tma = 0;
-        if (fmt == FMT_F16 && EPI != EPI_PARTIAL && src.g.out_planes && store_mode() && (src.g.out_nb32 & 1) == 0 &&
-            ((reinterpret_cast<uintptr_t>(src.g.out) | reinterpret_cast<uintptr_t>(src.g.out_lo)) & 127) == 0) {
+        // fp16 plane tiles leave the epilogue by TMA stores (the API checked yp / dxp against planes_aligned)
+        if (fmt == FMT_F16 && src.g.out_planes) {
           if ((rc = make_store_map(&pr.o_hi, src.g.out, src.g.M, src.g.out_nb32 / 2))) return rc;
           if ((rc = make_store_map(&pr.o_lo, src.g.out_lo, src.g.M, src.g.out_nb32 / 2))) return rc;
-          pr.g.out_tma = 1;
         }
         pr.g.a_mn = src.a.mn_major;
         pr.g.b_mn = src.b.mn_major;
@@ -1295,8 +1202,6 @@ static int build_groups(int fmt, const GemmDesc* d, int n, std::vector<G>& out, 
           return fail(ADN_ERR_UNSUPPORTED, "%s: %d work items exceed the decode range", what, pr.g.tiles * pr.g.splits);
         pr.g.inv_tiles = 1.0f / (float)pr.g.tiles;
         pr.g.inv_tiles_n = 1.0f / (float)pr.g.tiles_n;
-        pr.g.inv_tiles_m = 1.0f / (float)pr.g.tiles_m;
-        pr.g.m_fastest = item_order_m_fastest(pr.g);
         pr.g.ovf = g_ovf_addr;
         pr.item0 = items;
         items += pr.g.tiles_m * pr.g.tiles_n * pr.g.splits;

@@ -43,20 +43,6 @@ __device__ __forceinline__ void mma_f16_n64(float (&d)[32], uint64_t da, uint64_
 
 // D (+)= A B, tf32 operands (both K-major), K = 8
 
-__device__ __forceinline__ void mma_tf32_n16(float (&d)[8], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
-               "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1;\n\t}"
-               : ADN_D8(0)
-               : "l"(da), "l"(db), "r"(scale_d));
-}
-
-__device__ __forceinline__ void mma_tf32_n48(float (&d)[24], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
-               "wgmma.mma_async.sync.aligned.m64n48k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23}, %24, %25, p, 1, 1;\n\t}"
-               : ADN_D8(0), ADN_D8(8), ADN_D8(16)
-               : "l"(da), "l"(db), "r"(scale_d));
-}
-
 __device__ __forceinline__ void mma_tf32_n64(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
                "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1;\n\t}"

@@ -228,7 +228,8 @@ int adn_dense_bwd_p(const void* xp, const void* wp, const void* dzp, void* dxp, 
  * Grouped forms: the same layer wave of several subnetworks (all candidates of an AdaNet iteration consume
  * the same minibatch, adanet/core/iteration.py:185-192) in ONE persistent launch per GEMM kind, so launch,
  * prologue and pipeline fill/drain are paid once per wave and narrow candidates hide behind wide ones.
- * Each op is checked before anything is launched; ops must not alias each other's outputs.
+ * Each op is checked before anything is launched; ops must not alias each other's outputs.  An output plane
+ * buffer (yp, dxp) that is not aligned as the plane-tensor contract above asks is ADN_ERR_INVALID.
  */
 /* One more input piece of a multi-source forward op: planes xp [batch, in] and the matching rows of the layer's
  * kernel as their own planes wp [in, out].  A dense layer over concat([x_0, x_1, ...], axis=-1) with kernel

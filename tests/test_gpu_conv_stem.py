@@ -1,7 +1,6 @@
 """GPU tests of the SimpleCNN stem kernels, in BOTH plane formats: the wgmma 3xTF32 forward (default, F in {16, 32}),
 the exact-fp32 SIMT forward (ADN_CONV_PATH=simt, and every F = 48 / 64 shape), the SIMT backward (default, all eight
-(channels, filters) instantiations, staged and image-only), the wgmma backward (ADN_CONV_BWD_PATH=tcgen05, F = 16)
-and the fixed-order partial reduce.
+(channels, filters) instantiations, staged and image-only) and the fixed-order partial reduce.
 
 Every output is compared element by element with a float64 NumPy restatement of the stem that keeps all four conv
 values of every pooled window and the componentwise error bound of each.  The planes are decoded in NumPy from the
@@ -105,13 +104,6 @@ def _tc_fwd_supported(H, W, C, F):
   nbuf = 4 if F == 16 else 2
   smem = 1024 + 2 * KB * 4 * F * 128 + 2 * 2 * KB * 128 * 128 + nbuf * (H + 2) * (W + 2) * C * 4 + F * 4
   return smem <= 227 * 1024
-
-
-def _tc_bwd_supported(H, W, C, F):
-  """convtc::bwd_supported"""
-  if F != 16:
-    return False
-  return 1024 + 2 * (2 * 2 * 128 * 128 + 2 * 2 * 16 * C * 128) + 2 * (H + 2) * (W + 2) * C * 4 <= 227 * 1024
 
 
 def _simt_groups(C, F):
@@ -290,26 +282,14 @@ def _ref_bwd(xp, arg, g, H, W, F):
   return dk.reshape(-1), gg.sum(axis=(0, 1, 2)), ak.reshape(-1), np.abs(gg).sum(axis=(0, 1, 2))
 
 
-def _bwd_chain(path, B, H, W, C, F, sms):
-  """longest rounding chain of one dk / db element, and the unit roundoff it is counted in.
-     SIMT: a thread FMAs over its ceil(B / grid) images x PH rows x ceil(PW / G) pixels, then the G-group sum, then
-           conv_stem_reduce_kernel's lane stride over the grid = min(B, 4 SMs) partials (ceil(grid / 32)) and the
-           5-step shuffle tree.
-     wgmma: per tile of 64 pixels 3 x 64 exact products accumulate in the MMA (u = 2^-23 ASSUMED, see _fwd_bound),
-           then acc += d once per tile (ceil(B / grid) images x ceil(tiles / 2) tiles per warpgroup, grid = min(B,
-           SMs)), the 8-term fold (2 warpgroups x 4 positions), then the reduce over grid partials.  db: per builder
-           thread a chain over the same tiles, then the 128-term fold, then the reduce."""
+def _bwd_chain(B, H, W, C, F, sms):
+  """longest rounding chain of one dk / db element: a thread FMAs over its ceil(B / grid) images x PH rows x
+  ceil(PW / G) pixels, then the G-group sum, then conv_stem_reduce_kernel's lane stride over the grid = min(B, 4 SMs)
+  partials (ceil(grid / 32)) and the 5-step shuffle tree."""
   PH, PW = H // 2, W // 2
-  if path == "simt":
-    grid = min(B, 4 * sms)
-    G = _simt_groups(C, F)
-    n = -(-B // grid) * PH * -(-PW // G) + G + -(-grid // 32) + 5
-    return n, U, n
-  grid = min(B, sms)
-  tiles = -(-(PH * PW) // 64)
-  per = -(-B // grid) * -(-tiles // 2)
-  red = -(-grid // 32) + 5
-  return 3 * 64 + per + 8 + red, 2.0 ** -23, per + 128 + red
+  grid = min(B, 4 * sms)
+  G = _simt_groups(C, F)
+  return -(-B // grid) * PH * -(-PW // G) + G + -(-grid // 32) + 5
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -332,8 +312,7 @@ def _fwd(torch, _lib, lib, monkeypatch, path, xd, kd, bd, B, H, W, C, F):
   return planes, L, arg[:B * cols // 16 * 4].view(torch.int32).view(B, cols // 16)
 
 
-def _bwd(torch, _lib, lib, monkeypatch, path, xd, argw, gd, B, H, W, C, F):
-  monkeypatch.setenv("ADN_CONV_BWD_PATH", path)
+def _bwd(torch, _lib, lib, xd, argw, gd, B, H, W, C, F):
   ws_bytes = _lib.query(_lib.Q_CONV_STEM_BWD_WS, B, C, F)
   ws = _alloc(torch, ws_bytes, SENTINEL)
   nk = 9 * C * F
@@ -341,7 +320,7 @@ def _bwd(torch, _lib, lib, monkeypatch, path, xd, argw, gd, B, H, W, C, F):
   db = _alloc(torch, 4 * F, SENTINEL)
   _lib.check(lib.adn_conv_stem_bwd(xd.data_ptr(), argw.data_ptr(), gd.data_ptr(), dk.data_ptr(), db.data_ptr(), B, H, W,
                                    C, F, ws.data_ptr(), ws_bytes, _sp(torch)), "adn_conv_stem_bwd")
-  where = "bwd %s %dx%dx%d F%d B%d" % (path, H, W, C, F, B)
+  where = "bwd %dx%dx%d F%d B%d" % (H, W, C, F, B)
   _guard_ok(where + " workspace", ws, ws_bytes)
   _guard_ok(where + " dkernel", dk, 4 * nk)
   _guard_ok(where + " dbias", db, 4 * F)
@@ -352,12 +331,8 @@ def _fwd_paths(H, W, C, F):
   return ["simt"] + (["tc"] if _tc_fwd_supported(H, W, C, F) else [])
 
 
-def _bwd_paths(H, W, C, F):
-  return ["simt"] + (["tcgen05"] if _tc_bwd_supported(H, W, C, F) else [])
-
-
-def _run_random(torch, _lib, lib, monkeypatch, f16, B, H, W, C, F, seed, bwd_tc=True):
-  """random data: every forward path and every backward path against the fp64 bounds; determinism of both"""
+def _run_random(torch, _lib, lib, monkeypatch, f16, B, H, W, C, F, seed):
+  """random data: every forward path and the backward against the fp64 bounds; determinism of both"""
   rng = np.random.default_rng(seed)
   x = rng.uniform(0, 1, (B, H, W, C)).astype(F32)
   x[::2] -= 0.5                                   # some signed images as well
@@ -384,16 +359,13 @@ def _run_random(torch, _lib, lib, monkeypatch, f16, B, H, W, C, F, seed, bwd_tc=
   gd = torch.as_tensor(g).cuda()
   xp, _ = _patches(x)
   dk_ref, db_ref, ak, ab = _ref_bwd(xp, arg, g, H, W, F)
-  for path in _bwd_paths(H, W, C, F) if bwd_tc else ["simt"]:
-    dk, db = _bwd(torch, _lib, lib, monkeypatch, path, xd, argw, gd, B, H, W, C, F)
-    dk2, db2 = _bwd(torch, _lib, lib, monkeypatch, path, xd, argw, gd, B, H, W, C, F)
-    where = "bwd %s %dx%dx%d F%d B%d" % (path, H, W, C, F, B)
-    assert torch.equal(dk, dk2) and torch.equal(db, db2), "%s: two backward calls differ" % where
-    n, u, nb = _bwd_chain("simt" if path == "simt" else "tc", B, H, W, C, F, _sms(_lib))
-    rep = 0.0 if path == "simt" else 3.001 * 2.0 ** -22           # 3xTF32 representation error
-    _check(where + ": dkernel " + ("simt" if path == "simt" else "wgmma"), dk.cpu().numpy(), dk_ref,
-           (rep + _gamma(n, u) * 1.002) * ak)
-    _check(where + ": dbias " + ("simt" if path == "simt" else "wgmma"), db.cpu().numpy(), db_ref, _gamma(nb) * ab)
+  dk, db = _bwd(torch, _lib, lib, xd, argw, gd, B, H, W, C, F)
+  dk2, db2 = _bwd(torch, _lib, lib, xd, argw, gd, B, H, W, C, F)
+  where = "bwd %dx%dx%d F%d B%d" % (H, W, C, F, B)
+  assert torch.equal(dk, dk2) and torch.equal(db, db2), "%s: two backward calls differ" % where
+  n = _bwd_chain(B, H, W, C, F, _sms(_lib))
+  _check(where + ": dkernel simt", dk.cpu().numpy(), dk_ref, _gamma(n) * 1.002 * ak)
+  _check(where + ": dbias simt", db.cpu().numpy(), db_ref, _gamma(n) * ab)
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -410,7 +382,7 @@ def test_conv_stem_exact(env, monkeypatch, B, H, W, C, F):
   is a multiple of its quantum below 2^24 quanta, and every operand splits into TF32 with lo = 0, so every kernel is
   exact in any order.  The planes must be byte-identical to adn_planes_split of the exact pooled values, every sign
   bit and every arg-max (first maximum in scan order, decided here by many exact ties) exact, and dkernel / dbias of
-  both backward paths byte-identical to the exact sums."""
+  the backward byte-identical to the exact sums."""
   torch, _lib, lib, f16 = env
   rng = np.random.default_rng(1000 + B * H * W * C + F)
   x = (rng.integers(0, 3, (B, H, W, C)) / 2.0).astype(F32)
@@ -455,11 +427,10 @@ def test_conv_stem_exact(env, monkeypatch, B, H, W, C, F):
   gd = torch.as_tensor(g).cuda()
   want_dk, want_db = dk_ref.astype(F32), db_ref.astype(F32)
   assert np.array_equal(want_dk.astype(np.float64), dk_ref) and np.array_equal(want_db.astype(np.float64), db_ref)
-  for path in _bwd_paths(H, W, C, F):
-    dk, db = _bwd(torch, _lib, lib, monkeypatch, path, xd, argw, gd, B, H, W, C, F)
-    where = "exact bwd %s %dx%dx%d F%d B%d" % (path, H, W, C, F, B)
-    assert np.array_equal(dk.cpu().numpy().view(np.uint32), want_dk.view(np.uint32)), where + ": dkernel"
-    assert np.array_equal(db.cpu().numpy().view(np.uint32), want_db.view(np.uint32)), where + ": dbias"
+  dk, db = _bwd(torch, _lib, lib, xd, argw, gd, B, H, W, C, F)
+  where = "exact bwd %dx%dx%d F%d B%d" % (H, W, C, F, B)
+  assert np.array_equal(dk.cpu().numpy().view(np.uint32), want_dk.view(np.uint32)), where + ": dkernel"
+  assert np.array_equal(db.cpu().numpy().view(np.uint32), want_db.view(np.uint32)), where + ": dbias"
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -543,10 +514,10 @@ def test_conv_stem_beyond_2g_elements(env, monkeypatch):
     gd[torch.as_tensor(rows, device="cuda")] = torch.as_tensor(g).cuda()
     xp, _ = _patches(x)
     dk_ref, db_ref, ak, ab = _ref_bwd(xp, arg, g, H, W, F)
-    dk, db = _bwd(torch, _lib, lib, monkeypatch, "simt", xd, argw, gd, B, H, W, C, F)
-    n, u, nb = _bwd_chain("simt", B, H, W, C, F, _sms(_lib))
-    _check("2G bwd: dkernel simt", dk.cpu().numpy(), dk_ref, _gamma(n, u) * ak)
-    _check("2G bwd: dbias simt", db.cpu().numpy(), db_ref, _gamma(nb) * ab)
+    dk, db = _bwd(torch, _lib, lib, xd, argw, gd, B, H, W, C, F)
+    n = _bwd_chain(B, H, W, C, F, _sms(_lib))
+    _check("2G bwd: dkernel simt", dk.cpu().numpy(), dk_ref, _gamma(n) * ak)
+    _check("2G bwd: dbias simt", db.cpu().numpy(), db_ref, _gamma(n) * ab)
   finally:
     del xd
     torch.cuda.empty_cache()
@@ -576,25 +547,24 @@ def test_conv_stem_overflow_flag(env, monkeypatch, path):
 
 
 def _envelope_shapes():
-  out = [(64, 64, 3, 16), (96, 96, 1, 16), (48, 48, 3, 64), (28, 28, 1, 64), (32, 32, 3, 64)]
+  out = [(64, 64, 3, 16), (96, 96, 1, 16), (48, 48, 3, 64), (28, 28, 1, 64), (32, 32, 3, 64), (44, 44, 3, 16),
+         (46, 46, 3, 16), (100, 100, 1, 16), (102, 102, 1, 16)]
   for C in (1, 3):
     for F in (16, 32, 48, 64):
       h = _largest_square(C, F, lambda *a: True)
       out.append((h, h, C, F))                                  # 154 (C = 1) / 88 (C = 3)
       hb = _largest_square(C, F, _simt_bwd_staged)
       out += [(hb, hb, C, F), (hb + 2, hb + 2, C, F)]           # last staged / first image-only SIMT backward
-  for C in (1, 3):
-    h = _largest_square(C, 16, _tc_bwd_supported)
-    out += [(h, h, C, 16), (h + 2, h + 2, C, 16)]               # last wgmma backward / first fall-back
   out += [(152, 152, 1, 16), (86, 86, 3, 64), (2, 6142, 1, 64), (6142, 2, 1, 16), (2, 2046, 3, 16), (2046, 2, 3, 48)]
   return sorted(set(out))
 
 
-@pytest.mark.parametrize("bwd_path", ["simt", "tcgen05"])
+@pytest.mark.parametrize("fwd_path", ["simt", "tcgen05"])
 @pytest.mark.parametrize("H,W,C,F", _envelope_shapes())
-def test_conv_stem_envelope(env, monkeypatch, bwd_path, H, W, C, F):
-  """every shape the forward accepts, the backward accepts, on the default path and with the opt-in wgmma backward
-  (which falls back where it does not fit); and the result is right"""
+def test_conv_stem_envelope(env, monkeypatch, fwd_path, H, W, C, F):
+  """every shape the forward accepts, the backward accepts, routed by the arg-max words of either forward path
+  (ADN_CONV_PATH=simt, or the default wgmma forward, which falls back to SIMT where it does not fit); and the result
+  is right"""
   torch, _lib, lib, f16 = env
   assert _accepted(H, W, C, F)
   B = 2
@@ -604,20 +574,18 @@ def test_conv_stem_envelope(env, monkeypatch, bwd_path, H, W, C, F):
   bias = (rng.standard_normal(F) * 0.1).astype(F32)
   xd, kd, bd = (torch.as_tensor(a).cuda() for a in (x, k, bias))
   cols = (H // 2) * (W // 2) * F
-  planes, L, argw = _fwd(torch, _lib, lib, monkeypatch, "tc", xd, kd, bd, B, H, W, C, F)
+  planes, L, argw = _fwd(torch, _lib, lib, monkeypatch, fwd_path, xd, kd, bd, B, H, W, C, F)
   vals, _ = _decode(torch, planes, L)
   vals = vals[:, :cols]
   arg = _unpack_arg(argw.cpu().numpy(), cols)
   g = np.where(vals > 0, rng.standard_normal((B, cols)) / B, 0.0).astype(F32)
   gd = torch.as_tensor(g).cuda()
-  dk, db = _bwd(torch, _lib, lib, monkeypatch, bwd_path, xd, argw, gd, B, H, W, C, F)
+  dk, db = _bwd(torch, _lib, lib, xd, argw, gd, B, H, W, C, F)
   xp, _ = _patches(x)
   dk_ref, db_ref, ak, ab = _ref_bwd(xp, arg, g, H, W, F)
-  tc = bwd_path == "tcgen05" and _tc_bwd_supported(H, W, C, F)
-  n, u, nb = _bwd_chain("tc" if tc else "simt", B, H, W, C, F, _sms(_lib))
-  rep = 3.001 * 2.0 ** -22 if tc else 0.0
-  _check("envelope: dkernel " + ("wgmma" if tc else "simt"), dk.cpu().numpy(), dk_ref, (rep + _gamma(n, u) * 1.002) * ak)
-  _check("envelope: dbias " + ("wgmma" if tc else "simt"), db.cpu().numpy(), db_ref, _gamma(nb) * ab)
+  n = _bwd_chain(B, H, W, C, F, _sms(_lib))
+  _check("envelope: dkernel simt", dk.cpu().numpy(), dk_ref, _gamma(n) * 1.002 * ak)
+  _check("envelope: dbias simt", db.cpu().numpy(), db_ref, _gamma(n) * ab)
 
 
 @pytest.mark.parametrize("H,W,C,F", [(156, 156, 1, 16), (90, 90, 3, 64), (2, 6144, 1, 16), (2048, 2, 3, 32),
@@ -628,9 +596,8 @@ def test_conv_stem_rejects_outside_envelope(env, monkeypatch, H, W, C, F):
   p = t.data_ptr()
   assert not _accepted(H, W, C, F)
   want = ERR_INVALID if (H % 2 or W % 2) else ERR_UNSUPPORTED
-  for fwd_path, bwd_path in (("tc", "simt"), ("simt", "tcgen05")):
+  for fwd_path in ("tc", "simt"):
     monkeypatch.setenv("ADN_CONV_PATH", fwd_path)
-    monkeypatch.setenv("ADN_CONV_BWD_PATH", bwd_path)
     assert lib.adn_conv_stem_fwd(p, p, p, p, p, 2, H, W, C, F, _sp(torch)) == want
     assert lib.adn_conv_stem_bwd(p, p, p, p, p, 2, H, W, C, F, p, 1 << 18, _sp(torch)) == want
   assert (t == 0).all()

@@ -387,17 +387,14 @@ def test_nonfinite_opt_step_planes(env):
 
 
 def _conv_masks(img, g, arg, H, W, C, F):
-  """non-finite masks of dkernel [3,3,C,F] / dbias [F] of both backward formulations.  SIMT: dK[ky,kx,c,f] sums
-  patch(argmax)[ky,kx,c] * g over pooled pixels, so a non-finite pixel reaches the taps of the arg-max position only.
-  wgmma: dW' = A^T G' over the whole 4x4 patch, with G' zero at the three other positions, and 0 * NaN = NaN, so it
-  reaches the taps of all four positions."""
+  """non-finite masks of dkernel [3,3,C,F] / dbias [F] of the SIMT backward: dK[ky,kx,c,f] sums
+  patch(argmax)[ky,kx,c] * g over pooled pixels, so a non-finite pixel reaches the taps of the arg-max position only."""
   B = img.shape[0]
   PH, PW = H // 2, W // 2
   pad = np.zeros((B, H + 2, W + 2, C), dtype=bool)
   pad[:, 1:-1, 1:-1, :] = ~np.isfinite(img)
   gnf = ~np.isfinite(g.reshape(B, PH * PW, F))
   simt = np.zeros((3, 3, C, F), dtype=bool)
-  tc = np.zeros((3, 3, C, F), dtype=bool)
   for b in range(B):
     for p in range(PH * PW):
       py, px = divmod(p, PW)
@@ -408,17 +405,12 @@ def _conv_masks(img, g, arg, H, W, C, F):
         simt[:, :, :, f] |= pad[b, 2 * py + dy: 2 * py + dy + 3, 2 * px + dx: 2 * px + dx + 3, :]
         if gnf[b, p, f]:
           simt[:, :, :, f] = True
-          tc[:, :, :, f] = True
-      for pos in range(4):
-        dy, dx = pos >> 1, pos & 1
-        tc |= pad[b, 2 * py + dy: 2 * py + dy + 3, 2 * px + dx: 2 * px + dx + 3, :][..., None]
-  return simt, tc, gnf.any(axis=(0, 1))
+  return simt, gnf.any(axis=(0, 1))
 
 
 @pytest.mark.parametrize("case", ["pixel", "dpooled"])
-def test_nonfinite_conv_stem_bwd(env, monkeypatch, case):
-  """A NaN pixel / NaN dpooled entry through both backward variants.  A NaN in dpooled reaches the same outputs on
-  both; a NaN pixel reaches more taps on the wgmma variant (see _conv_masks)."""
+def test_nonfinite_conv_stem_bwd(env, case):
+  """A NaN pixel / NaN dpooled entry through the backward reaches exactly the outputs _conv_masks predicts."""
   torch, _lib, lib = env
   B, H, W, C, F = 3, 10, 10, 3, 16
   cols = (H // 2) * (W // 2) * F
@@ -432,24 +424,16 @@ def test_nonfinite_conv_stem_bwd(env, monkeypatch, case):
   else:
     g[2, 7 * F + 3] = _from_bits([0x7FFFFFFF])[0]
     g[0, 11 * F + 9] = _from_bits([0xFFFFFFFF])[0]
-  simt_m, tc_m, db_m = _conv_masks(img, g, arg, H, W, C, F)
+  simt_m, db_m = _conv_masks(img, g, arg, H, W, C, F)
   assert simt_m.any() and not simt_m.all()
   xd, gd, ad = _dev(torch, img), _dev(torch, g), _dev(torch, arg.view(np.int32))
-  out = {}
-  for path in ("simt", "tcgen05"):
-    monkeypatch.setenv("ADN_CONV_BWD_PATH", path)
-    wsb = _lib.query(_lib.Q_CONV_STEM_BWD_WS, B, C, F)
-    ws = torch.full((wsb,), 0xFF, dtype=torch.uint8, device="cuda")
-    dk, db = _nan(torch, 9 * C * F), _nan(torch, F)
-    _lib.check(lib.adn_conv_stem_bwd(xd.data_ptr(), ad.data_ptr(), gd.data_ptr(), dk.data_ptr(), db.data_ptr(), B, H, W,
-                                     C, F, ws.data_ptr(), wsb, _sp(torch)), "adn_conv_stem_bwd " + path)
-    out[path] = (dk.cpu().numpy().reshape(3, 3, C, F), db.cpu().numpy())
-  assert np.array_equal(~np.isfinite(out["simt"][0]), simt_m)
-  assert np.array_equal(~np.isfinite(out["tcgen05"][0]), tc_m)
-  for path in out:
-    assert np.array_equal(~np.isfinite(out[path][1]), db_m), path
-  if case == "dpooled":
-    assert np.array_equal(simt_m, tc_m)
+  wsb = _lib.query(_lib.Q_CONV_STEM_BWD_WS, B, C, F)
+  ws = torch.full((wsb,), 0xFF, dtype=torch.uint8, device="cuda")
+  dk, db = _nan(torch, 9 * C * F), _nan(torch, F)
+  _lib.check(lib.adn_conv_stem_bwd(xd.data_ptr(), ad.data_ptr(), gd.data_ptr(), dk.data_ptr(), db.data_ptr(), B, H, W,
+                                   C, F, ws.data_ptr(), wsb, _sp(torch)), "adn_conv_stem_bwd")
+  assert np.array_equal(~np.isfinite(dk.cpu().numpy().reshape(3, 3, C, F)), simt_m)
+  assert np.array_equal(~np.isfinite(db.cpu().numpy()), db_m)
 
 
 # ------------------------------------------------------------------------------------------------------------------

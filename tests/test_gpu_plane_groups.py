@@ -11,14 +11,7 @@ Bounds are componentwise: |err_ij| <= 3e-6 * (|A| |B|)_ij (+ 3e-6 |b_j| for a bi
 of the magnitudes.  A normwise bound against the largest entry cannot see a wrong small entry.  Operand entries are
 drawn with magnitudes in [0.5, 2): in the fp16 format every operand then stays in fp16's normal range, where a plane
 pair carries 22 significant bits (include/adanet_b200.h).
-
-dump_cases() runs a fixed set of groups and writes every output buffer as raw bytes.  A child process runs it again
-under each process-static A/B switch (ADN_PL_TMA_STORE=0, ADN_PL_MFAST=1), and the outputs must be byte-identical.
 """
-
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -27,7 +20,6 @@ from tests.test_gpu_planes import _layout, _merge, _planes
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 TOL = 3e-6
 ERR_WORKSPACE, ERR_UNSUPPORTED = -12, -95
 DX_MUL = float(np.float32(1.0 / (1.0 - 0.25)))      # the dropout backward below a rate-0.25 layer
@@ -597,63 +589,3 @@ def test_tf32_power_of_two_rows_commute(env):
   for a, b in zip(*res):
     assert np.array_equal(a * e, b)
 
-
-# ------------------------------------------------------------------------------------------------------------------
-# process-static A/B switches
-# ------------------------------------------------------------------------------------------------------------------
-def dump_cases(out_dir, formats=("f16", "tf32")):
-  """Runs a fixed set of forward and backward groups in each plane format and writes every output buffer as raw
-  bytes to out_dir/<format>_<case>_<op>_<output>.bin.  Leaves the plane format as it found it."""
-  torch, _lib, lib = _open()
-  os.makedirs(out_dir, exist_ok=True)
-  before = _lib.plane_format()
-
-  def put(tag, t):
-    torch.cuda.synchronize()
-    with open(os.path.join(out_dir, tag + ".bin"), "wb") as fh:
-      fh.write(t.cpu().numpy().tobytes())
-
-  try:
-    for fmt in formats:
-      _set_format(_lib, fmt)
-      for name, spec, B in (("g11", FWD_G11, 129), ("wrap", FWD_WRAP, 128)):
-        case = _fwd_case(torch, _lib, lib, B, spec, seed=B * 31 + len(spec))
-        for k, buf in enumerate(_fwd_run(torch, _lib, lib, case, list(range(len(spec))))):
-          put("%s_fwd-%s_%d_y" % (fmt, name, k), buf)
-      for B in (256, 8192):
-        case = _bwd_case(torch, _lib, lib, B, BWD_OPS, seed=B + 17)
-        for k, f in enumerate(_bwd_run(torch, _lib, lib, case, list(range(len(BWD_OPS))))):
-          for key in ("dw", "dxp", "dx", "cs"):
-            if f[key] is not None:
-              put("%s_bwd-b%d_%d_%s" % (fmt, B, k, key), f[key])
-  finally:
-    _lib.set_plane_format(before)
-
-
-@pytest.fixture(scope="module")
-def default_dump(tmp_path_factory):
-  out = tmp_path_factory.mktemp("default")
-  dump_cases(str(out))
-  return out
-
-
-@pytest.mark.parametrize("switch", ["ADN_PL_TMA_STORE=0", "ADN_PL_MFAST=1"])
-def test_process_static_switch(default_dump, tmp_path, switch):
-  """ADN_PL_TMA_STORE=0 (fp16 planes leave the epilogue by direct stores instead of TMA) and ADN_PL_MFAST=1 (row
-  blocks fastest in the work-item order) are read once per process.  Both leave every byte of every output
-  unchanged: the direct stores convert with the same __floats2half2_rn, and the item order does not touch the
-  arithmetic of a tile."""
-  key, val = switch.split("=")
-  env = dict(os.environ)
-  env.pop("ADN_PL_TMA_STORE", None)
-  env.pop("ADN_PL_MFAST", None)
-  env[key] = val
-  code = "import sys; sys.path.insert(0, %r); from tests.test_gpu_plane_groups import dump_cases; dump_cases(sys.argv[1])" % ROOT
-  cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + ["-c", code, str(tmp_path)]
-  r = subprocess.run(cmd, env=env, cwd=ROOT, capture_output=True, text=True, timeout=900)
-  assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-4000:]
-  want = sorted(os.listdir(default_dump))
-  assert sorted(os.listdir(tmp_path)) == want and want
-  differ = [n for n in want
-            if (default_dump / n).read_bytes() != (tmp_path / n).read_bytes()]
-  assert not differ, "%s changes %d outputs: %s" % (switch, len(differ), differ[:10])

@@ -185,6 +185,14 @@ def _check_head_and_plane_validation(lib):
   bwd_p(INVALID, "bad shape", in_=0)
   bwd_p(INVALID, "dz_log2_scale", dz=-61)
 
+  # an output plane buffer off the alignment the TMA stores need, here at a 64 B offset
+  fwd_p(INVALID, "yp: plane buffers must be 256 B aligned", yp=P + 64)
+  bwd_p(INVALID, "dxp: plane buffers must be 256 B aligned", dxp=P + 64)
+  fop = _lib.FwdOp(xp=P, wp=P, yp=P + 64, in_=64, out=32)
+  rejects("adn_dense_fwd_p_group", INVALID, "yp: plane buffers must be 256 B aligned", ctypes.byref(fop), 1, 256, None)
+  bop = _lib.BwdOp(xp=P, wp=P, dzp=P, dxp=P + 64, dw=P, in_=64, out=32, x_relu_mask=1, workspace=P, workspace_bytes=BIG)
+  rejects("adn_dense_bwd_p_group", INVALID, "dxp: plane buffers must be 256 B aligned", ctypes.byref(bop), 1, 256, None)
+
   rejects("adn_colsum", INVALID, "null pointer", None, 256, 10, P, P, BIG, None)
   rejects("adn_colsum", INVALID, "null pointer", P, 256, 10, P, None, BIG, None)
   rejects("adn_colsum", INVALID, "bad shape", P, 0, 10, P, P, BIG, None)
