@@ -183,6 +183,12 @@ __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.a
 __device__ __forceinline__ void sts_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
   asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
 }
+__device__ __forceinline__ void sts_v2(uint32_t addr, float a, float b) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
+}
+__device__ __forceinline__ void lds_v4(uint32_t addr, float& a, float& b, float& c, float& d) {
+  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(a), "=f"(b), "=f"(c), "=f"(d) : "r"(addr) : "memory");
+}
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
@@ -248,9 +254,8 @@ __device__ __forceinline__ void store_row32_tf32(const GemmParams& g, const floa
 // The hi and lo' planes have a slab each, and every slice commits its hi store and then its lo' store, so before a
 // slab is written `wait_group.read 1` only waits for the store issued from it one slice earlier, not for the one
 // just issued.
-__device__ __forceinline__ void store_slice_tma(const CUtensorMap* o_hi, const CUtensorMap* o_lo, uint32_t slab_hi,
-                                                uint32_t slab_lo, const float* a, int lane, int mrow0, int cbase) {
-  uint32_t w[16], lw[16];
+// 32 values -> their fp16 hi and lo' plane words, two values per word
+__device__ __forceinline__ void split_f16x32(const float* a, uint32_t (&w)[16], uint32_t (&lw)[16]) {
 #pragma unroll
   for (int q = 0; q < 16; ++q) {
     const __half2 h2 = __floats2half2_rn(a[2 * q], a[2 * q + 1]);
@@ -259,6 +264,11 @@ __device__ __forceinline__ void store_slice_tma(const CUtensorMap* o_hi, const C
     w[q] = *reinterpret_cast<const uint32_t*>(&h2);
     lw[q] = *reinterpret_cast<const uint32_t*>(&l2);
   }
+}
+__device__ __forceinline__ void store_slice_tma(const CUtensorMap* o_hi, const CUtensorMap* o_lo, uint32_t slab_hi,
+                                                uint32_t slab_lo, const float* a, int lane, int mrow0, int cbase) {
+  uint32_t w[16], lw[16];
+  split_f16x32(a, w, lw);
   const uint32_t roff = (uint32_t)lane * 64u, sw = ((uint32_t)lane >> 1) & 3u;
   if (lane == 0) bulk_wait_read1();        // the hi store of the previous slice has read slab_hi
   __syncwarp();
@@ -285,11 +295,11 @@ __device__ __forceinline__ void store_slice_tma(const CUtensorMap* o_hi, const C
 // Forward epilogue with planes out, WITHOUT a register transpose: lane = row keeps its 32 accumulators (bias already
 // added by the caller), applies ReLU / dropout, forms the sign-bit word, splits pairs of values with packed conversions
 // and hands its 32 columns of each plane to the slab + TMA store path (fp16) or writes them with direct 16 B stores
-// (TF32: 128 B per plane).
-template <int FMT>
+// (TF32: 128 B per plane).  A caller with its own fp16 store path passes it as `store16` (the maps and slabs unused).
+template <int FMT, class Store16 = void>
 __device__ __forceinline__ void emit_slice_fwd_planes(const GemmParams& g, float* a, uint32_t drop_step, int lane, int mrow0,
                                                       int cbase, const CUtensorMap* o_hi, const CUtensorMap* o_lo,
-                                                      uint32_t slab_hi, uint32_t slab_lo) {
+                                                      uint32_t slab_hi, uint32_t slab_lo, const Store16* store16 = nullptr) {
   const int my_row = mrow0 + lane;
   const int kbo = cbase >> 5;
   if (kbo >= g.out_nb32) return;                         // warp-uniform
@@ -315,7 +325,8 @@ __device__ __forceinline__ void emit_slice_fwd_planes(const GemmParams& g, float
     for (int j = 0; j < 32; ++j)
       if (!((cmask >> j) & 1u)) a[j] = 0.f;
   }
-  if (FMT == FMT_F16) store_slice_tma(o_hi, o_lo, slab_hi, slab_lo, a, lane, mrow0, cbase);
+  if constexpr (!std::is_void<Store16>::value) (*store16)(a);
+  else if (FMT == FMT_F16) store_slice_tma(o_hi, o_lo, slab_hi, slab_lo, a, lane, mrow0, cbase);
   else if (my_row < g.M) store_row32_tf32(g, a, my_row, cbase);
   uint32_t bits = 0u;
 #pragma unroll
@@ -338,14 +349,14 @@ __device__ __forceinline__ void colsum_round(float* a, int lane) {
 }
 
 // dX epilogue with planes out, without a register transpose: sign-bit ReLU mask, plane stores as in the forward
-// epilogue (slab + TMA for fp16, direct stores from the row-owning lane for TF32), and the per-32-row column sums
+// epilogue (slab + TMA for fp16 or the caller's `store16`, direct stores from the row-owning lane for TF32), and the per-32-row column sums
 // (the bias gradient of the layer below) by a butterfly over the warp: at distance w a lane keeps the half of its
 // columns selected by bit w of its lane id and receives the partner's partial sums for them, so after five rounds
 // lane l holds the sum of column l over the 32 rows (31 shuffles and adds per lane, fixed order).
-template <int FMT>
+template <int FMT, class Store16 = void>
 __device__ __forceinline__ void emit_slice_mask_planes(const GemmParams& g, float* a, uint32_t mwq, int lane, int mrow0, int cbase,
                                                        const CUtensorMap* o_hi, const CUtensorMap* o_lo, uint32_t slab_hi,
-                                                       uint32_t slab_lo) {
+                                                       uint32_t slab_lo, const Store16* store16 = nullptr) {
   const int my_row = mrow0 + lane;
   const int kbo = cbase >> 5;
   if (kbo >= g.out_nb32) return;                         // warp-uniform
@@ -360,7 +371,8 @@ __device__ __forceinline__ void emit_slice_mask_planes(const GemmParams& g, floa
     for (int j = 0; j < 32; ++j)
       if (!((keep >> j) & 1u)) a[j] = 0.f;
   }
-  if (FMT == FMT_F16) store_slice_tma(o_hi, o_lo, slab_hi, slab_lo, a, lane, mrow0, cbase);
+  if constexpr (!std::is_void<Store16>::value) (*store16)(a);
+  else if (FMT == FMT_F16) store_slice_tma(o_hi, o_lo, slab_hi, slab_lo, a, lane, mrow0, cbase);
   else if (my_row < g.M) store_row32_tf32(g, a, my_row, cbase);
   if (g.colsum_part) {
     colsum_round<16>(a, lane);
@@ -589,10 +601,11 @@ __device__ __forceinline__ void fold_chunk(float (&acc)[32], const float (&H)[32
 // One k-block of a consumer warpgroup on fp16 planes: 4 K steps of 16, each hi*hi into H and hi*lo' + lo'*hi into S
 // (first: the chunk starts, the MMAs overwrite H and S).  The warpgroup's 64 A rows start 8 KiB into the A tiles in
 // both majornesses; a K step advances 32 B inside a K-major 128 B row, 16 rows of 128 B in an MN-major tile.
+// a_hi: the warpgroup's 64 rows of the A hi tile, with the lo' tile A_TILE after it; b_hi: the B hi tile, with the
+// lo' tile B_TILE after it.
 template <int A_MN, int B_MN>
-__device__ __forceinline__ void f16_kblock(uint32_t st, int wgi, float (&H)[32], float (&S)[32], bool first) {
-  const uint32_t a_hi = st + (uint32_t)wgi * 8192u, a_lo = a_hi + A_TILE;
-  const uint32_t b_hi = st + 2 * A_TILE, b_lo = b_hi + B_TILE;
+__device__ __forceinline__ void f16_kblock_at(uint32_t a_hi, uint32_t b_hi, float (&H)[32], float (&S)[32], bool first) {
+  const uint32_t a_lo = a_hi + A_TILE, b_lo = b_hi + B_TILE;
   constexpr uint32_t a_step = A_MN ? 2048u : 32u, b_step = B_MN ? 2048u : 32u;
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
@@ -603,6 +616,11 @@ __device__ __forceinline__ void f16_kblock(uint32_t st, int wgi, float (&H)[32],
     wg::mma_f16_n64<A_MN, B_MN>(S, dah, dbl, sd);
     wg::mma_f16_n64<A_MN, B_MN>(S, dal, dbh, 1u);
   }
+}
+// the same on one pipeline stage of pl_gemm_kernel (A_hi A_lo B_hi B_lo)
+template <int A_MN, int B_MN>
+__device__ __forceinline__ void f16_kblock(uint32_t st, int wgi, float (&H)[32], float (&S)[32], bool first) {
+  f16_kblock_at<A_MN, B_MN>(st + (uint32_t)wgi * 8192u, st + 2 * A_TILE, H, S, first);
 }
 
 // byte offset of (row r, byte c) in a tile of 128 B rows written by TMA with SWIZZLE_128B (16 B chunk ^= row % 8)
@@ -873,6 +891,216 @@ pl_gemm_ms_kernel(const __grid_constant__ MsGroup grp) {
 }
 
 // ---------------------------------------------------------------------------------
+// Thin-K kernel (pl_thin_kernel): fp16 planes in and out, every problem one accumulation chunk (K <= 128) and one
+// split -- the first-layer forward and the logits layer's dX of a training step.  Their tiles have one or two k-blocks
+// of MMA work and a full epilogue each, so pl_gemm_kernel's single epilogue warpgroup sets their pace and its ring
+// reloads the same A rows for every tile.  Here a work item is (problem, 128-row block, a run of up to THIN_RUN
+// N tiles): the row block's A planes are loaded into shared memory once per item and the B tiles stream through a
+// small ring.  Each tile is two units of 64 rows; unit u of the CTA goes to math warpgroup u % THIN_WGS, which runs
+// its MMAs, folds them, transposes the result through its own staging area and emits it, one 32 x 32 slice per warp,
+// with the functions pl_gemm_kernel's epilogue uses; each plane of the unit then leaves in one 64 x 64 TMA store.  The arithmetic is the same instruction sequence (bias start,
+// f16_kblock, fold_chunk), the dropout hash is keyed by element index and the column sums are written per 32-row
+// slice, so the results are bit-identical to pl_gemm_kernel's.  One producer warp issues the TMA loads.
+// ---------------------------------------------------------------------------------
+static constexpr int THIN_WGS = 3;                    // math warpgroups
+static constexpr int THIN_THREADS = 128 * THIN_WGS + 32;
+static constexpr int THIN_RUN = 4;                    // N tiles per work item at most (load balance)
+static constexpr int THIN_STAGES = 2;
+static constexpr int THIN_A_BYTES = Fmt<FMT_F16>::CHUNK * 2 * A_TILE;     // per k-block: A_hi, A_lo (128 rows)
+static constexpr int THIN_B_STAGE = Fmt<FMT_F16>::CHUNK * 2 * B_TILE;     // per k-block: B_hi, B_lo (64 columns)
+static constexpr int THIN_ACC_FLOATS = 64 * BN;                           // one warpgroup's 64 x 64 staging area
+static constexpr int THIN_SLAB_WG = 2 * 64 * 128;                        // a warpgroup's hi and lo' [64][64] fp16 slabs
+static constexpr int THIN_SLAB_BYTES = THIN_WGS * THIN_SLAB_WG;
+static constexpr int THIN_SMEM_BYTES =
+    1024 + THIN_A_BYTES + THIN_STAGES * THIN_B_STAGE + THIN_WGS * THIN_ACC_FLOATS * 4 + THIN_SLAB_BYTES + BAR_BYTES;
+static_assert(THIN_SMEM_BYTES <= 232448, "shared memory per block");
+
+// work items of one problem: 128-row blocks x runs of N tiles
+__host__ __device__ __forceinline__ int thin_runs(int tiles_n) { return (tiles_n + THIN_RUN - 1) / THIN_RUN; }
+
+template <int EPI>
+__global__ void __launch_bounds__(THIN_THREADS, 1)
+pl_thin_kernel(const __grid_constant__ Group grp) {
+  constexpr int A_MN = 0, B_MN = EPI == EPI_BIAS_ACT;   // fwd: A K-major, B MN-major; dX: both K-major
+  constexpr int BK = Fmt<FMT_F16>::BK;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  const uint32_t a_smem = smem_u32(smem);
+  const uint32_t b_smem = a_smem + THIN_A_BYTES;
+  float* acc_stage = reinterpret_cast<float*>(smem + THIN_A_BYTES + THIN_STAGES * THIN_B_STAGE);
+  float* slabs = acc_stage + THIN_WGS * THIN_ACC_FLOATS;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(slabs) + THIN_SLAB_BYTES);
+  uint64_t* full_bar = bars;                       // [THIN_STAGES]  B tile loaded
+  uint64_t* empty_bar = bars + THIN_STAGES;        // [THIN_STAGES]  both 64-row units of the tile done, count 8 warps
+  uint64_t* a_full = bars + 2 * THIN_STAGES;       // the item's A rows loaded
+  uint64_t* a_empty = a_full + 1;                  // every math warp done with them, count 4 THIN_WGS
+
+  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
+  const int lane = threadIdx.x & 31;
+  const int n_items = grp.total_items;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < THIN_STAGES; ++s) {
+      mbar_init(smem_u32(&full_bar[s]), 1);
+      mbar_init(smem_u32(&empty_bar[s]), 8);
+    }
+    mbar_init(smem_u32(a_full), 1);
+    mbar_init(smem_u32(a_empty), 4 * THIN_WGS);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  if (warp == 4 * THIN_WGS && lane < grp.n) {
+    tma_prefetch_desc(&grp.p[lane].a_hi);
+    tma_prefetch_desc(&grp.p[lane].a_lo);
+    tma_prefetch_desc(&grp.p[lane].b_hi);
+    tma_prefetch_desc(&grp.p[lane].b_lo);
+  }
+  __syncthreads();
+
+  if (warp == 4 * THIN_WGS) {
+    // ================= TMA producer =================
+    if (lane == 0) {
+      int cur = 0, next0 = first_next0(grp);
+      uint32_t tile = 0, icount = 0;               // B tiles and items of this CTA so far
+      for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++icount) {
+        cur = find_problem(grp, cur, item, next0);
+        const Problem& pr = grp.p[cur];
+        const GemmParams& g = pr.g;
+        const int runs = thin_runs(g.tiles_n), local = item - pr.item0;
+        const int mb = local / runs, t0 = (local - mb * runs) * THIN_RUN;
+        const int nt = min(THIN_RUN, g.tiles_n - t0);
+        if (icount > 0) mbar_wait(smem_u32(a_empty), (icount - 1) & 1u);
+        mbar_expect_tx(smem_u32(a_full), g.total_kb * 2 * A_TILE);
+        for (int kb = 0; kb < g.total_kb; ++kb) {
+          tma_load_3d(&pr.a_hi, smem_u32(a_full), a_smem + kb * 2 * A_TILE, 0, mb * BM, kb);
+          tma_load_3d(&pr.a_lo, smem_u32(a_full), a_smem + kb * 2 * A_TILE + A_TILE, 0, mb * BM, kb);
+        }
+        for (int j = 0; j < nt; ++j, ++tile) {
+          const uint32_t s = tile % THIN_STAGES, ph = (tile / THIN_STAGES) & 1u;
+          mbar_wait(smem_u32(&empty_bar[s]), ph ^ 1u);
+          const uint32_t fb = smem_u32(&full_bar[s]);
+          mbar_expect_tx(fb, g.total_kb * 2 * B_TILE);
+          const int n0 = (t0 + j) * BN;
+          for (int kb = 0; kb < g.total_kb; ++kb) {
+            const uint32_t dst = b_smem + s * THIN_B_STAGE + kb * 2 * B_TILE;
+            const int b1 = B_MN ? kb * BK : n0, b2 = B_MN ? (n0 / BK) : kb;
+            tma_load_3d(&pr.b_hi, fb, dst, 0, b1, b2);
+            tma_load_3d(&pr.b_lo, fb, dst + B_TILE, 0, b1, b2);
+          }
+        }
+      }
+    }
+    return;
+  }
+
+  // ================= math warpgroups =================
+  const int wgi = warp >> 2, wq = warp & 3;
+  const int gid = lane >> 2, tq = lane & 3;        // accumulator fragment coordinates
+  const uint32_t stage = smem_u32(acc_stage + wgi * THIN_ACC_FLOATS);
+  const uint32_t slab_hi = smem_u32(slabs) + (uint32_t)wgi * THIN_SLAB_WG, slab_lo = slab_hi + THIN_SLAB_WG / 2;
+  const int srow = 32 * (wq >> 1) + lane, scol = 32 * (wq & 1);   // this warp's slice of the 64 x 64 unit
+  int cur = 0, next0 = first_next0(grp);
+  uint32_t tile = 0, icount = 0;                   // B tiles and items of this CTA so far (2 tile 64-row units)
+  for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++icount) {
+    cur = find_problem(grp, cur, item, next0);
+    const Problem& pr = grp.p[cur];
+    const GemmParams& g = pr.g;
+    const int runs = thin_runs(g.tiles_n), local = item - pr.item0;
+    const int mb = local / runs, t0 = (local - mb * runs) * THIN_RUN;
+    const int nt = min(THIN_RUN, g.tiles_n - t0);
+    // this warpgroup's units of the item: u0, u0 + THIN_WGS, ... < 2 nt
+    const int u0 = (int)((wgi + THIN_WGS - 2 * tile % THIN_WGS) % THIN_WGS);
+    mbar_wait(smem_u32(a_full), icount & 1u);
+    if (u0 >= 2 * nt && lane == 0) mbar_arrive(smem_u32(a_empty));
+    for (int u = u0; u < 2 * nt; u += THIN_WGS) {
+      const int j = u >> 1, half = u & 1;
+      const uint32_t t = tile + j, s = t % THIN_STAGES;
+      const int n0 = (t0 + j) * BN;
+      // dX: the ReLU-mask word of the lane's row, loaded before the MMAs (all ones without a mask, 0 past M)
+      uint32_t mw = 0xffffffffu;
+      if (EPI == EPI_MASK && g.mask_bits) {
+        const int my_row = mb * BM + 64 * half + srow, kbo = (n0 + scol) >> 5;
+        mw = (my_row < g.M && kbo < g.out_nb32) ? __ldg(g.mask_bits + (size_t)kbo * g.M + my_row) : 0u;
+      }
+      mbar_wait(smem_u32(&full_bar[s]), (t / THIN_STAGES) & 1u);
+      // MMA accumulators of this unit only: nothing keeps them live through the epilogue (4 warps of a quadrant
+      // share its registers at THIN_THREADS, so a thread has 128)
+      float H[32], S[32];
+#pragma unroll
+      for (int jj = 0; jj < 32; ++jj) H[jj] = S[jj] = 0.f;
+      wg::fence_regs(H);
+      wg::fence_regs(S);
+      wg::fence();
+      const uint32_t a_st = a_smem + half * 8192u, b_st = b_smem + s * THIN_B_STAGE;
+      f16_kblock_at<A_MN, B_MN>(a_st, b_st, H, S, true);
+      if (g.total_kb > 1) f16_kblock_at<A_MN, B_MN>(a_st + 2 * A_TILE, b_st + 2 * B_TILE, H, S, false);
+      wg::commit();
+      wg::wait<0>();
+      wg::fence_regs(H);
+      wg::fence_regs(S);
+      __syncwarp();
+      if (lane == 0) {
+        mbar_arrive(smem_u32(&empty_bar[s]));
+        if (u + THIN_WGS >= 2 * nt) mbar_arrive(smem_u32(a_empty));   // this warp's last MMA on the item's A rows
+      }
+      float acc[32];
+      const int c0 = n0 + 2 * tq;
+      const float* bias = (EPI == EPI_BIAS_ACT && g.bias) ? g.bias + c0 : nullptr;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {       // the bias starts the accumulation
+          const int dc = 8 * jj + (e & 1);
+          acc[4 * jj + e] = (bias && c0 + dc < g.N) ? __ldg(bias + dc) : 0.f;
+        }
+      fold_chunk<FMT_F16>(acc, H, S);
+      // fragment layout -> staging area -> row per lane.  Past this barrier the warpgroup's previous slices have been
+      // read, and its previous tile stores have read the slabs (the issuing thread waited for them).
+      if (wq == 0 && lane == 0) bulk_wait_read0();
+      asm volatile("bar.sync %0, 128;" ::"r"(1 + wgi) : "memory");
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) {   // 32-bit shared addresses: 64-bit generic ones for every store ran out of registers
+        const int row = 16 * wq + gid, col = 8 * jj + 2 * tq;
+        sts_v2(stage + 4u * acc_off(row, col), acc[4 * jj], acc[4 * jj + 1]);
+        sts_v2(stage + 4u * acc_off(row + 8, col), acc[4 * jj + 2], acc[4 * jj + 3]);
+      }
+      asm volatile("bar.sync %0, 128;" ::"r"(1 + wgi) : "memory");
+      float a[32];
+#pragma unroll
+      for (int q = 0; q < 8; ++q) lds_v4(stage + 4u * acc_off(srow, scol + 4 * q), a[4 * q], a[4 * q + 1], a[4 * q + 2], a[4 * q + 3]);
+      // the lane's row of each plane goes into the warpgroup's [64 rows][128 B] slabs (16 B chunk ^= row % 8, the
+      // SWIZZLE_128B layout); one thread then stores the 64 x 64 unit of each plane with a single TMA store, 128 B
+      // per row, instead of four 32 x 32 boxes of 64 B rows per plane
+      const auto store16 = [&](const float* v) {
+        uint32_t w[16], lw[16];
+        split_f16x32(v, w, lw);
+        const uint32_t roff = (uint32_t)srow * 128u, sw = (uint32_t)srow & 7u, c0 = (uint32_t)scol >> 3;
+#pragma unroll
+        for (uint32_t q = 0; q < 4; ++q) {
+          sts_v4(slab_hi + roff + (((c0 + q) ^ sw) << 4), w[4 * q], w[4 * q + 1], w[4 * q + 2], w[4 * q + 3]);
+          sts_v4(slab_lo + roff + (((c0 + q) ^ sw) << 4), lw[4 * q], lw[4 * q + 1], lw[4 * q + 2], lw[4 * q + 3]);
+        }
+      };
+      const int mrow0 = mb * BM + 64 * half + 32 * (wq >> 1), cbase = n0 + scol;
+      if (EPI == EPI_BIAS_ACT) {
+        const uint32_t drop_step = g.drop_thresh != 0u ? (uint32_t)(*g.drop_step) : 0u;
+        emit_slice_fwd_planes<FMT_F16>(g, a, drop_step, lane, mrow0, cbase, nullptr, nullptr, 0u, 0u, &store16);
+      }
+      else
+        emit_slice_mask_planes<FMT_F16>(g, a, mw, lane, mrow0, cbase, nullptr, nullptr, 0u, 0u, &store16);
+      fence_async_smem();
+      asm volatile("bar.sync %0, 128;" ::"r"(1 + wgi) : "memory");
+      if (wq == 0 && lane == 0) {
+        tma_store_3d(&pr.o_hi, slab_hi, 0, mb * BM + 64 * half, n0 / BK);
+        tma_store_3d(&pr.o_lo, slab_lo, 0, mb * BM + 64 * half, n0 / BK);
+        bulk_commit();
+      }
+    }
+    tile += nt;
+  }
+  if (wq == 0 && lane == 0) bulk_wait0();    // stores complete before the CTA (and its shared memory) goes away
+}
+
+// ---------------------------------------------------------------------------------
 // dense <-> planes conversion (inputs x / labels-side gradients / weights; everything
 // between two GEMMs is written as planes by the producing epilogue instead)
 // ---------------------------------------------------------------------------------
@@ -1010,6 +1238,8 @@ int init() {
 #undef ADN_PL_ATTR
     ok = ok && cudaFuncSetAttribute(pl_gemm_ms_kernel<FMT_TF32>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) == cudaSuccess;
     ok = ok && cudaFuncSetAttribute(pl_gemm_ms_kernel<FMT_F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) == cudaSuccess;
+    ok = ok && cudaFuncSetAttribute(pl_thin_kernel<EPI_BIAS_ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, THIN_SMEM_BYTES) == cudaSuccess;
+    ok = ok && cudaFuncSetAttribute(pl_thin_kernel<EPI_MASK>, cudaFuncAttributeMaxDynamicSharedMemorySize, THIN_SMEM_BYTES) == cudaSuccess;
     if (!ok) {
       (void)cudaGetLastError();
       rc = fail(ADN_ERR_CUDA, "pl::init: cudaFuncSetAttribute(smem=%d) failed", SMEM_BYTES);
@@ -1098,10 +1328,11 @@ static int make_map(int fmt, CUtensorMap* map, const void* plane, int64_t rows, 
   return ADN_OK;
 }
 
-// output planes (fp16) as TMA store targets: [32 columns (64 B)][32 rows] boxes, SWIZZLE_64B in shared memory
-static int make_store_map(CUtensorMap* map, const void* plane, int64_t rows, int64_t nkb) {
+// output planes (fp16) as TMA store targets: [box columns][box rows] boxes; box = 32 (pl_gemm_kernel's 32 x 32 slices,
+// 64 B rows, SWIZZLE_64B in shared memory) or 64 (pl_thin_kernel's 64 x 64 units, 128 B rows, SWIZZLE_128B)
+static int make_store_map(CUtensorMap* map, const void* plane, int64_t rows, int64_t nkb, int box_rc = 32) {
   if (!g_encode) return fail(ADN_ERR_CUDA, "pl: adn_init() was not called");
-  const MapKey key{plane, rows, nkb, 2, FMT_F16};      // mn = 2: the store box
+  const MapKey key{plane, rows, nkb, 2, FMT_F16, box_rc};      // mn = 2: a store box
   {
     std::lock_guard<std::mutex> lk(g_map_mu);
     auto it = g_maps.find(key);
@@ -1113,10 +1344,11 @@ static int make_store_map(CUtensorMap* map, const void* plane, int64_t rows, int
   }
   cuuint64_t gdim[3] = {64u, (cuuint64_t)rows, (cuuint64_t)nkb};
   cuuint64_t gstride[2] = {128u, (cuuint64_t)rows * 128u};
-  cuuint32_t box[3] = {32u, 32u, 1u};
+  cuuint32_t box[3] = {(cuuint32_t)box_rc, (cuuint32_t)box_rc, 1u};
   cuuint32_t estr[3] = {1u, 1u, 1u};
   CUresult r = g_encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(plane), gdim, gstride, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
+                        CU_TENSOR_MAP_INTERLEAVE_NONE, box_rc == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
+                        CU_TENSOR_MAP_L2_PROMOTION_NONE,
                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail(ADN_ERR_CUDA, "cuTensorMapEncodeTiled (store box) failed (%d) rows=%lld nkb=%lld", (int)r,
                                      (long long)rows, (long long)nkb);
@@ -1146,6 +1378,15 @@ static int encode_maps(int fmt, const GemmDesc& d, CUtensorMap* a_hi, CUtensorMa
   return ADN_OK;
 }
 
+// A group runs on pl_thin_kernel when every problem is one fp16 accumulation chunk with planes out and no split.
+static bool thin_group(int fmt, const Group& grp) {
+  if (fmt != FMT_F16) return false;
+  for (int i = 0; i < grp.n; ++i) {
+    const GemmParams& g = grp.p[i].g;
+    if (!g.out_planes || g.splits != 1 || g.total_kb > Fmt<FMT_F16>::CHUNK) return false;
+  }
+  return true;
+}
 template <int FMT, int EPI>
 static void launch_kernel(const Group& grp, int grid, cudaStream_t st) {
   pl_gemm_kernel<FMT, EPI><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(grp);
@@ -1208,6 +1449,20 @@ static int build_groups(int fmt, const GemmDesc* d, int n, std::vector<G>& out, 
       }
       grp.n = m;
       grp.total_items = items;
+      if constexpr (!MS) {
+        if (thin_group(fmt, grp)) {     // pl_thin_kernel's work items (128-row block x run of THIN_RUN N tiles) and store boxes
+          items = 0;
+          for (int i = 0; i < m; ++i) {
+            Problem& pr = grp.p[i];
+            pr.item0 = items;
+            items += pr.g.tiles_m * thin_runs(pr.g.tiles_n);
+            int rc;
+            if ((rc = make_store_map(&pr.o_hi, pr.g.out, pr.g.M, pr.g.out_nb32 / 2, 64))) return rc;
+            if ((rc = make_store_map(&pr.o_lo, pr.g.out_lo, pr.g.M, pr.g.out_nb32 / 2, 64))) return rc;
+          }
+          grp.total_items = items;
+        }
+      }
     }
   }
   return ADN_OK;
@@ -1219,6 +1474,8 @@ static int launch_groups(int fmt, const std::vector<G>& groups, cudaStream_t st,
     if constexpr (std::is_same<G, MsGroup>::value) {
       if (fmt == FMT_F16) pl_gemm_ms_kernel<FMT_F16><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(grp);
       else pl_gemm_ms_kernel<FMT_TF32><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(grp);
+    } else if (thin_group(fmt, grp)) {
+      if constexpr (EPI != EPI_PARTIAL) pl_thin_kernel<EPI><<<grid, THIN_THREADS, THIN_SMEM_BYTES, st>>>(grp);
     } else {
       if (fmt == FMT_F16) launch_kernel<FMT_F16, EPI>(grp, grid, st);
       else launch_kernel<FMT_TF32, EPI>(grp, grid, st);

@@ -71,6 +71,9 @@ def classify(name):
   m = re.search(r"pl_gemm_kernel<(\d+), (\d+)>", name)
   if m:
     return "gemm", int(m.group(2))
+  m = re.search(r"pl_thin_kernel<(\d+)>", name)
+  if m:
+    return "gemm", int(m.group(1))
   for key, kind in (("reduce_partials", "reduce"), ("colsum", "colsum"), ("opt_step", "optimizer"),
                     ("step_increment", "optimizer"), ("split_kernel", "split"), ("head_bookkeeping", "bookkeeping"),
                     ("counter_add", "counter")):
