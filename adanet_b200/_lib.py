@@ -24,7 +24,7 @@ PATH_AUTO, PATH_SIMT, PATH_TCGEN05 = 0, 1, 2
 PLANES_TF32, PLANES_F16 = 0, 1
 (Q_VERSION, Q_DENSE_BWD_WS, Q_HEAD_WS, Q_DENSE_FWD_PATH, Q_SM_COUNT, Q_LAUNCH_COUNT, Q_DENSE_BWD_PATH,
  Q_DENSE_FWD_WS, Q_PLANES_BYTES, Q_DENSE_BWD_P_WS, Q_COLSUM_WS, Q_CONV_STEM_BWD_WS, Q_PLANE_FORMAT,
- Q_TMA_MAP_CACHE_HITS, Q_TMA_MAP_CACHE_MISSES) = range(15)
+ Q_TMA_MAP_CACHE_HITS, Q_TMA_MAP_CACHE_MISSES, Q_HEAD_PATH, Q_HEAD_WIDE_WS) = range(17)
 
 EXPORTS = (
     "adn_last_error", "adn_init", "adn_query", "adn_set_dense_path", "adn_dense_fwd", "adn_dense_bwd", "adn_head_loss",
@@ -33,6 +33,7 @@ EXPORTS = (
     "adn_opt_step_p", "adn_head_loss_p", "adn_dense_fwd_p_group", "adn_dense_bwd_p_group",
     "adn_l1_grad_add", "adn_conv_stem_fwd", "adn_conv_stem_bwd", "adn_set_plane_format", "adn_plane_overflow",
     "adn_planes_split_scaled", "adn_head_group", "adn_head_bookkeeping", "adn_opt_step_group",
+    "adn_head_group_wide",
 )
 
 
@@ -136,6 +137,7 @@ def load():
   lib.adn_opt_step_p.argtypes = [c_int, POINTER(p), POINTER(p), POINTER(p), POINTER(p), POINTER(i64), c_int,
                                  POINTER(f32), p, POINTER(p), POINTER(i64), p]
   lib.adn_head_group.argtypes = [POINTER(HeadOp), c_int, i64, i64, p]
+  lib.adn_head_group_wide.argtypes = [POINTER(HeadOp), c_int, i64, i64, p]
   lib.adn_head_bookkeeping.argtypes = [POINTER(HeadBook), c_int, p, p]
   lib.adn_opt_step_group.argtypes = [POINTER(OptOp), c_int, p]
   for name in EXPORTS:

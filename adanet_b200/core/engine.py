@@ -17,7 +17,7 @@ schedule (IterationPlan._enqueue_waves) of grouped launches built from one op
 builder per stage:
 
   forward layer   -> DenseNet.fwd_op          in adn_dense_fwd_p_group (frozen members too: _fwd_waves)
-  losses, heads   -> CandidatePlan.sub_head_op / EnsembleHead.head_op in adn_head_group
+  losses, heads   -> CandidatePlan.sub_head_op / EnsembleHead.head_op in adn_head_group(_wide) (launch_heads)
   backward layer  -> CandidatePlan.bwd_op     in adn_dense_bwd_p_group
   optimizers      -> _Optimizer.op            in adn_opt_step_group
   EMA / trace     -> EnsembleHead.book        in adn_head_bookkeeping
@@ -87,17 +87,49 @@ def _metric_value(metric: str, out3: torch.Tensor, ens_logits: Optional[torch.Te
   return float(out3[2 if metric == "adanet_loss" else 0].item())
 
 
+MAX_HEAD_DIM = 16384        # widest head adn_head_group_wide runs
+
+
+def check_head_dim(logits_dim: int):
+  """Refuses, when a plan is built, a head wider than any head kernel runs."""
+  if not 1 <= logits_dim <= MAX_HEAD_DIM:
+    raise NotImplementedError("heads of %d logits: the head kernels run 1..%d" % (logits_dim, MAX_HEAD_DIM))
+
+
+def _head_wide(logits_dim: int, n_members: int) -> bool:
+  """True when a head of `n_members` members runs on adn_head_group_wide (ADN_Q_HEAD_PATH)."""
+  return _lib.query(_lib.Q_HEAD_PATH, logits_dim, n_members) == 1
+
+
+def head_ws_bytes(rows: int, logits_dim: int, n_members: int) -> int:
+  """Workspace of one head op on the kernel its shape runs on."""
+  q = _lib.Q_HEAD_WIDE_WS if _head_wide(logits_dim, n_members) else _lib.Q_HEAD_WS
+  return _lib.query(q, rows, logits_dim, n_members)
+
+
 def _check_head_ws(rows: int, logits_dim: int, n_members: int, have: int):
   """A head launched on the first `rows` examples of buffers sized for the static batch must fit the workspace
   allocated for that batch."""
-  need = _lib.query(_lib.Q_HEAD_WS, rows, logits_dim, n_members)
+  need = head_ws_bytes(rows, logits_dim, n_members)
   if need > have:
     raise RuntimeError("head workspace of %d bytes is too small for %d rows (needs %d)" % (have, rows, need))
 
 
+def launch_heads(lib, ops: Sequence["_lib.HeadOp"], rows: int, dim: int, sp: int):
+  """Every head launch of the engine: the ops that fit adn_head_group go there, the others to adn_head_group_wide,
+  each in its given order."""
+  narrow = [o for o in ops if not _head_wide(dim, o.n_members)]
+  wide = [o for o in ops if _head_wide(dim, o.n_members)]
+  if narrow:
+    _lib.check(lib.adn_head_group((_lib.HeadOp * len(narrow))(*narrow), len(narrow), rows, dim, sp), "adn_head_group")
+  if wide:
+    _lib.check(lib.adn_head_group_wide((_lib.HeadOp * len(wide))(*wide), len(wide), rows, dim, sp),
+               "adn_head_group_wide")
+
+
 def _run_head(lib, op: "_lib.HeadOp", rows: int, dim: int, sp: int):
-  """One head op on its own: a one-op adn_head_group over `rows` examples."""
-  _lib.check(lib.adn_head_group((_lib.HeadOp * 1)(op), 1, rows, dim, sp), "adn_head_group")
+  """One head op on its own."""
+  launch_heads(lib, [op], rows, dim, sp)
 
 
 def _load_rows(x_buf: torch.Tensor, labels_buf: Optional[torch.Tensor], x, y) -> int:
@@ -673,6 +705,7 @@ class EnsembleHead:
     """`alloc(shape)`: where the tensors that a row-sharded candidate averages across ranks are placed (its
     _GradArena); `row0`: first minibatch row of this head when `batch` is a row slice -- members built for the full
     minibatch (frozen ones) are then read from that row on."""
+    check_head_dim(logits_dim)
     self.lib, self.name, self.ens = lib, name, ens
     self.batch, self.C, self.head = batch, logits_dim, _HEAD_KIND[head]
     self.member_nets = list(member_nets)
@@ -762,7 +795,7 @@ class EnsembleHead:
     self.decay = float(decay)
     self.trace = torch.zeros((trace_capacity, 4), **f32)
     self.trace_capacity = trace_capacity
-    self.head_ws_bytes = _lib.query(_lib.Q_HEAD_WS, batch, logits_dim, n_members)
+    self.head_ws_bytes = head_ws_bytes(batch, logits_dim, n_members)
     self.head_ws = torch.empty((self.head_ws_bytes,), dtype=torch.uint8, device=device)
     if self.mix == _lib.MIX_MATRIX:
       self._members = _lib.ptr_array([t.data_ptr() for t in self.mw_logits])
@@ -961,7 +994,7 @@ class CandidatePlan:
       self.dz = [torch.empty((batch, hid), **f32) for _ in range(2)] if hid else []
       # `workspace` serves the backward and the subnetwork's own head loss, one after the other on its stream
       ws_bytes = max(_lib.query(_lib.Q_DENSE_BWD_WS, batch, dims[i], dims[i + 1]) for i in range(len(dims) - 1))
-    ws_bytes = max(ws_bytes, _lib.query(_lib.Q_HEAD_WS, batch, logits_dim, 1))
+    ws_bytes = max(ws_bytes, head_ws_bytes(batch, logits_dim, 1))
     self.workspace = torch.empty((ws_bytes,), dtype=torch.uint8, device=device)
     self.ws_bytes = ws_bytes
     self.sub_out3 = galloc((3,)).zero_()           # {loss, -, -} of the subnetwork's own head
@@ -1186,6 +1219,7 @@ class IterationPlan:
     only its own heads warm-start from `prev_mixture_weights` / `prev_bias`.
     `shards[global candidate index]`: that candidate is row-sharded over the ranks of the ShardComm and this rank trains
     its slice of the minibatch rows (distributed/exchange.sharded_placement)."""
+    check_head_dim(logits_dim)
     self.lib = _require_cuda()
     self.device = device or torch.device("cuda", torch.cuda.current_device())
     self.iteration, self.batch, self.in_dim, self.C, self.head = iteration, batch, in_dim, logits_dim, head
@@ -1343,7 +1377,7 @@ class IterationPlan:
       _fwd_waves(lib, [(c.net, c.xp_own, c.batch, self.step_dev, 0) for c in bag], sp)
       own = self.labels is not None
       ops = [c.sub_head_op(c.labels_own if own else None, None if own else c.labels_own, c.own_out3) for c in bag]
-      _lib.check(lib.adn_head_group((_lib.HeadOp * len(ops))(*ops), len(ops), self.batch, self.C, sp), "adn_head_group")
+      launch_heads(lib, ops, self.batch, self.C, sp)
       self._bwd_waves(bag, lambda c: c.xp_own, sp)
       for c in bag:
         if c.net.stem:
@@ -1374,8 +1408,7 @@ class IterationPlan:
     hops = [(c.sub_head_op(self.labels, self.labels_f, c.sub_out3), c.batch) for c in self.candidates]
     hops += [(h.head_op(self.labels, self.labels_f), h.batch) for _, h, _ in self.heads if h.groupable]
     for bsz in sorted({b for _, b in hops}, reverse=True):
-      ops = [o for o, b in hops if b == bsz]
-      _lib.check(lib.adn_head_group((_lib.HeadOp * len(ops))(*ops), len(ops), bsz, self.C, sp), "adn_head_group")
+      launch_heads(lib, [o for o, b in hops if b == bsz], bsz, self.C, sp)
     for _, h, _ in self.heads:
       if not h.groupable:
         h.enqueue_matrix(self.labels, self.labels_f, sp, self.xp)

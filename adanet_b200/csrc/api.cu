@@ -53,6 +53,8 @@ int dense_path() {
 }
 
 int64_t head_workspace_bytes_public(int64_t batch, int64_t dim, int64_t members);
+int64_t head_wide_workspace_bytes_public(int64_t batch, int64_t dim, int64_t members);
+int head_path(int64_t dim, int64_t members);
 int heads_init();
 
 }  // namespace adn
@@ -110,6 +112,8 @@ extern "C" int adn_query(int key, int64_t a, int64_t b, int64_t c, int64_t* out_
       *out_host = (pick_fwd_path(a, b, c) == ADN_PATH_TCGEN05) ? tc::dense_fwd_workspace_bytes(a, b, c) : 0;
       return ADN_OK;
     case ADN_Q_HEAD_WORKSPACE_BYTES: *out_host = head_workspace_bytes_public(a, b, c) + 256; return ADN_OK;
+    case ADN_Q_HEAD_PATH: *out_host = head_path(a, b); return ADN_OK;
+    case ADN_Q_HEAD_WIDE_WORKSPACE_BYTES: *out_host = head_wide_workspace_bytes_public(a, b, c) + 256; return ADN_OK;
     case ADN_Q_DENSE_FWD_PATH: *out_host = pick_fwd_path(a, b, c); return ADN_OK;
     case ADN_Q_DENSE_BWD_PATH: *out_host = pick_bwd_path(a, b, c); return ADN_OK;
     case ADN_Q_SM_COUNT: *out_host = sm_count(); return ADN_OK;

@@ -4,7 +4,10 @@
 // coalesced float4 loads over the flat [rows*dim] tile of each member.
 // Every head entry point (adn_head_group, adn_ensemble_head, adn_head_loss(_p))
 // goes through one validator (head_group_op) and one launcher (run_heads) of one
-// kernel family: a single head is a one-op group.
+// kernel family: a single head is a one-op group.  adn_head_group_wide runs the
+// same ops through the same validator on a second kernel that keeps no copy of
+// the members in shared memory, for heads the first one cannot hold (dim > 64,
+// or members x dim past its slab); both share the finalize.
 //
 // Reference arithmetic being replaced (file:line in tensorflow/adanet v0.9.0):
 //   weighted logits / sum    adanet/ensemble/weighted.py:433-453,545-561
@@ -23,6 +26,13 @@ namespace adn {
 static constexpr int kRows = 128;       // rows (examples) per CTA == threads per CTA
 static constexpr int kMaxMembers = 64;
 static constexpr int kMaxDim = 64;
+static constexpr size_t kHeadSmemMax = 227 * 1024;
+// wide kernel (adn_head_group_wide)
+static constexpr int kWThreads = 256;
+static constexpr int kWMaxDim = 16384;
+static constexpr int kWMaxRows = 32;              // rows per row block
+static constexpr int kWRowBytes = 96 * 1024;      // smem for the row block's gradient rows: two CTAs per SM
+static constexpr int kWMaxCta = 512;
 
 struct HeadParams {
   const float* members[kMaxMembers];
@@ -51,6 +61,8 @@ struct HeadParams {
   float* out3;
   float* dw;
   float* dbias;
+  // wide kernel only (wide_geom): rows per row block, row blocks per CTA, smem row stride, 16 B loads allowed
+  int rb, bpc, ld, vec;
 };
 
 __device__ __forceinline__ float weight_of(const HeadParams& p, int k, int c) {
@@ -349,6 +361,252 @@ ensemble_finalize_group_kernel(const __grid_constant__ HeadGroup g) {
   finalize_body(p, p.part, p.n_cta);
 }
 
+// ---- wide heads: any dim up to kWMaxDim, no per-member smem slab ----
+// Four consecutive columns [c, c + nv) of a row: one 16 B load when `vec` (dim % 4 == 0 and aligned bases), else scalar
+// loads of the nv <= 4 valid columns.  Either way the same elements land in the same lanes, so the arithmetic below
+// does not depend on the alignment.
+__device__ __forceinline__ float4 wide_ld4(const float* p, int nv, int vec) {
+  if (vec) return __ldg(reinterpret_cast<const float4*>(p));
+  float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+  v.x = __ldg(p);
+  if (nv > 1) v.y = __ldg(p + 1);
+  if (nv > 2) v.z = __ldg(p + 2);
+  if (nv > 3) v.w = __ldg(p + 3);
+  return v;
+}
+__device__ __forceinline__ void wide_st4(float* p, float4 v, int nv, int vec) {
+  if (vec) {
+    *reinterpret_cast<float4*>(p) = v;
+    return;
+  }
+  p[0] = v.x;
+  if (nv > 1) p[1] = v.y;
+  if (nv > 2) p[2] = v.z;
+  if (nv > 3) p[3] = v.w;
+}
+__device__ __forceinline__ float warp_sum_xor(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+// One CTA = p.bpc consecutive row blocks of p.rb rows (the last CTA may own fewer; p.n_cta of them per op).
+// Row phase: warp w takes rows w, w + 8, ... of the block; lane l owns the 4-column chunks l, l + 32, ... of the row:
+// ens = bias + sum_k w_k (.) m_k in member order (one read of each member element from DRAM), then the head's loss
+// and dLoss/d(ens) = g into the block's smem row (softmax: row max, then the sum of exponentials).  Per-row sums are a
+// lane-sequential sum and a fixed xor tree.  Column phase: thread t owns columns t, t + 256, ... and adds the block's g
+// rows in row order into the CTA's accumulators (dbias, VECTOR dw from an L2 re-read of the member rows; SCALAR dw from
+// per-row dot products the row phase left in smem).  The accumulators live in the CTA's own contiguous slice of the
+// workspace and are moved to the output-major partials the finalize reads once the CTA is done.  Every order depends
+// only on (batch, dim, n_members).
+// smem: g[rb][ld] | rowdot[rb][kMaxMembers] | wloss[kWThreads / 32]
+__global__ void __launch_bounds__(kWThreads, 2)
+ensemble_head_wide_kernel(const __grid_constant__ HeadGroup grp) {
+  extern __shared__ __align__(16) float smem[];
+  const HeadParams& p = grp.p[blockIdx.y];
+  const int cta = blockIdx.x;
+  if (cta >= p.n_cta) return;
+  const int C = p.dim, N = p.n_members, ld = p.ld, rb = p.rb, vec = p.vec;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  constexpr int kWarps = kWThreads / 32;
+  float* grow = smem;
+  float* rowdot = grow + (size_t)rb * ld;
+  float* wloss = rowdot + (size_t)rb * kMaxMembers;
+  const bool want_dw = p.want_grads && !(p.mixture == ADN_MIX_MATRIX || p.colsum_only);
+  const bool scalar_dw = want_dw && p.mixture == ADN_MIX_SCALAR;
+  const bool vector_dw = want_dw && p.mixture == ADN_MIX_VECTOR;
+  const bool unit_w = p.mixture == ADN_MIX_MATRIX || p.w == nullptr;
+  const int nch = (C + 3) >> 2;
+  const float invb = 1.f / (float)p.batch, invn = 1.f / ((float)p.batch * (float)C);
+  float* acc = p.part + (size_t)p.n_out * p.n_cta + (size_t)cta * p.n_out;   // this CTA's accumulators [n_out]
+  const int64_t n_blocks = (p.batch + rb - 1) / rb;
+  const int64_t b0 = (int64_t)cta * p.bpc, b1 = min(b0 + p.bpc, n_blocks);
+  float wl = 0.f;                    // this warp's loss over its rows, row order
+
+  for (int64_t blk = b0; blk < b1; ++blk) {
+    const int64_t row0 = blk * rb;
+    const int nrows = (int)min((int64_t)rb, p.batch - row0);
+    // ---- row phase ----
+    for (int s = warp; s < nrows; s += kWarps) {
+      const int64_t r = row0 + s;
+      const size_t roff = (size_t)r * C;
+      float* e = grow + (size_t)s * ld;
+      float mx = -INFINITY, lsum = 0.f;
+      for (int i = lane; i < nch; i += 32) {
+        const int c = i * 4, nv = min(4, C - c);
+        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (p.bias) v = wide_ld4(p.bias + c, nv, 0);
+#pragma unroll 4
+        for (int k = 0; k < N; ++k) {
+          const float4 m = wide_ld4(p.members[k] + roff + c, nv, vec);
+          float4 wk = make_float4(1.f, 1.f, 1.f, 1.f);
+          if (!unit_w) {
+            if (p.mixture == ADN_MIX_SCALAR) {
+              const float ws = __ldg(p.w + k);
+              wk = make_float4(ws, ws, ws, ws);
+            } else {
+              wk = wide_ld4(p.w + (size_t)k * C + c, nv, vec);
+            }
+          }
+          v.x += wk.x * m.x;
+          v.y += wk.y * m.y;
+          v.z += wk.z * m.z;
+          v.w += wk.w * m.w;
+        }
+        if (p.ens_out) wide_st4(p.ens_out + roff + c, v, nv, vec);
+        float a[4] = {v.x, v.y, v.z, v.w};
+        if (p.head == ADN_HEAD_SOFTMAX_XENT) {
+#pragma unroll
+          for (int q = 0; q < 4; ++q)
+            if (q < nv) mx = fmaxf(mx, a[q]);
+        } else {
+          const float4 z4 = wide_ld4(p.labels_f + roff + c, nv, vec);
+          const float z[4] = {z4.x, z4.y, z4.z, z4.w};
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            if (q >= nv) {
+              a[q] = 0.f;
+              continue;
+            }
+            if (p.head == ADN_HEAD_MSE) {
+              const float d = a[q] - z[q];
+              lsum += d * d;
+              a[q] = 2.f * d * invn;
+            } else {
+              const float x = a[q];
+              lsum += fmaxf(x, 0.f) - x * z[q] + log1pf(expf(-fabsf(x)));
+              a[q] = (1.f / (1.f + expf(-x)) - z[q]) * invn;
+            }
+          }
+        }
+        *reinterpret_cast<float4*>(e + c) = make_float4(a[0], a[1], a[2], a[3]);
+      }
+      if (p.head == ADN_HEAD_SOFTMAX_XENT) {
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+        const int y = (int)p.labels[r];
+        __syncwarp();
+        const float zy = e[y] - mx;
+        __syncwarp();
+        float sx = 0.f;
+        for (int i = lane; i < nch; i += 32) {
+          const int c = i * 4, nv = min(4, C - c);
+          float4 v = *reinterpret_cast<float4*>(e + c);
+          v.x = expf(v.x - mx);
+          v.y = nv > 1 ? expf(v.y - mx) : 0.f;
+          v.z = nv > 2 ? expf(v.z - mx) : 0.f;
+          v.w = nv > 3 ? expf(v.w - mx) : 0.f;
+          sx += v.x;
+          sx += v.y;
+          sx += v.z;
+          sx += v.w;
+          *reinterpret_cast<float4*>(e + c) = v;
+        }
+        sx = warp_sum_xor(sx);
+        lsum = -(zy - logf(sx));
+        const float inv = 1.f / sx;
+        for (int i = lane; i < nch; i += 32) {
+          const int c = i * 4, nv = min(4, C - c);
+          float4 v = *reinterpret_cast<float4*>(e + c);
+          v.x = (v.x * inv - (c == y ? 1.f : 0.f)) * invb;
+          v.y = nv > 1 ? (v.y * inv - (c + 1 == y ? 1.f : 0.f)) * invb : 0.f;
+          v.z = nv > 2 ? (v.z * inv - (c + 2 == y ? 1.f : 0.f)) * invb : 0.f;
+          v.w = nv > 3 ? (v.w * inv - (c + 3 == y ? 1.f : 0.f)) * invb : 0.f;
+          *reinterpret_cast<float4*>(e + c) = v;
+        }
+      } else {
+        lsum = warp_sum_xor(lsum);
+      }
+      wl += lsum;
+      if (p.dens) {
+        for (int i = lane; i < nch; i += 32) {
+          const int c = i * 4, nv = min(4, C - c);
+          wide_st4(p.dens + roff + c, *reinterpret_cast<const float4*>(e + c), nv, vec);
+        }
+      }
+      if (scalar_dw) {
+        // g_r . m_k per member (member row re-read from L2)
+        for (int k = 0; k < N; ++k) {
+          float d = 0.f;
+          for (int i = lane; i < nch; i += 32) {
+            const int c = i * 4, nv = min(4, C - c);
+            const float4 m = wide_ld4(p.members[k] + roff + c, nv, vec);
+            const float4 g = *reinterpret_cast<const float4*>(e + c);
+            d += g.x * m.x;
+            d += g.y * m.y;
+            d += g.z * m.z;
+            d += g.w * m.w;
+          }
+          d = warp_sum_xor(d);
+          if (lane == 0) rowdot[s * kMaxMembers + k] = d;
+        }
+      }
+    }
+    __syncthreads();
+    // ---- planes of g * dens_scale, zero padding columns up to the last k-block ----
+    if (p.densp.hi) {
+      const int pc8 = (p.dens_nkb * pl::fmt_bk(p.densp.fmt)) >> 3;
+      for (int i = tid; i < nrows * pc8; i += kWThreads) {
+        const int s = i / pc8, c8 = i - s * pc8;
+        const float* e = grow + (size_t)s * ld;
+        float m8[8];
+#pragma unroll
+        for (int q = 0; q < 8; ++q) {
+          const int c = c8 * 8 + q;
+          m8[q] = (c < C) ? e[c] * p.dens_scale : 0.f;
+        }
+        pl::plane_store8(p.densp, row0 + s, (int64_t)c8 * 8, m8, p.ovf);
+      }
+    }
+    // ---- column phase: block sums in row order, added to the CTA's accumulators ----
+    if (p.want_grads) {
+      const bool first = blk == b0;
+      for (int c = tid; c < C; c += kWThreads) {
+        float t = 0.f;
+        for (int s = 0; s < nrows; ++s) t += grow[(size_t)s * ld + c];
+        acc[1 + c] = first ? t : acc[1 + c] + t;
+        if (vector_dw) {
+          for (int k = 0; k < N; ++k) {
+            const float* mk = p.members[k] + (size_t)row0 * C + c;
+            float d = 0.f;
+            for (int s = 0; s < nrows; ++s) d += grow[(size_t)s * ld + c] * __ldg(mk + (size_t)s * C);
+            float* a = acc + 1 + C + (size_t)k * C + c;
+            *a = first ? d : *a + d;
+          }
+        }
+      }
+      if (scalar_dw) {
+        for (int k = tid; k < N; k += kWThreads) {
+          float d = 0.f;
+          for (int s = 0; s < nrows; ++s) d += rowdot[s * kMaxMembers + k];
+          acc[1 + C + k] = first ? d : acc[1 + C + k] + d;
+        }
+      }
+    }
+    __syncthreads();                 // the next block rewrites the smem rows
+  }
+
+  // ---- this CTA's partials, output-major (part[j * n_cta + cta]); each thread moves the accumulators it wrote ----
+  float* part = p.part + cta;
+  const size_t ps = (size_t)p.n_cta;
+  if (lane == 0) wloss[warp] = wl;
+  __syncthreads();
+  if (tid == 0) {
+    float t = 0.f;
+#pragma unroll
+    for (int w = 0; w < kWarps; ++w) t += wloss[w];
+    part[0] = t;
+  }
+  if (!p.want_grads) return;
+  for (int c = tid; c < C; c += kWThreads) {
+    part[(1 + c) * ps] = acc[1 + c];
+    if (vector_dw)
+      for (int k = 0; k < N; ++k) part[(1 + C + (size_t)k * C + c) * ps] = acc[1 + C + (size_t)k * C + c];
+  }
+  if (scalar_dw)
+    for (int k = tid; k < N; k += kWThreads) part[(1 + C + k) * ps] = acc[1 + C + k];
+}
+
 __device__ __forceinline__ void ema_update(float* state, const float* loss, float decay);
 // Per-step bookkeeping of every candidate ensemble in one launch (thread j = head j): zero-debiased EMA of its
 // adanet loss (candidate.py:117-129) and its row of the loss trace {sub_loss, ens_loss, adanet_loss, ema}
@@ -414,6 +672,41 @@ static size_t head_smem_bytes(int dim, int members) {
   return ((size_t)(members + 1) * kRows * dim + (size_t)(kRows / 32) * wr) * sizeof(float);
 }
 
+// 0: the op runs on adn_head_group (dim <= 64 and its member slab fits shared memory), 1: on adn_head_group_wide
+int head_path(int64_t dim, int64_t members) {
+  return (dim >= 1 && dim <= kMaxDim && members >= 1 && members <= kMaxMembers &&
+          head_smem_bytes((int)dim, (int)members) <= kHeadSmemMax) ? 0 : 1;
+}
+
+// Wide kernel geometry, a function of (batch, dim, members) alone: row blocks of rb rows (as many as kWRowBytes of
+// gradient rows hold, up to kWMaxRows), split into n_cta runs of bpc consecutive blocks.  The CTA cap keeps the
+// workspace (2 x n_out floats per CTA) near 32 MB for the widest heads and the finalize on one level.
+struct WideGeom {
+  int rb, ld, bpc, n_cta;
+  int64_t cta_cap;       // n_cta never exceeds it, for this batch or any smaller one
+};
+static WideGeom wide_geom(int64_t batch, int64_t dim, int64_t members) {
+  WideGeom g;
+  g.ld = (int)align_up(dim, 4);
+  g.rb = (int)std::max<int64_t>(1, std::min<int64_t>(kWMaxRows, kWRowBytes / (g.ld * (int64_t)sizeof(float))));
+  const int64_t n_blocks = ceil_div(batch, g.rb);
+  const int64_t n_out = 1 + dim + members * dim;
+  const int64_t cap = std::max<int64_t>(64, std::min<int64_t>(kWMaxCta, (int64_t(1) << 22) / n_out));
+  g.cta_cap = std::min(n_blocks, cap);
+  g.bpc = (int)ceil_div(n_blocks, g.cta_cap);
+  g.n_cta = (int)ceil_div(n_blocks, g.bpc);
+  return g;
+}
+// partials [n_out][n_cta] | per-CTA accumulators [n_cta][n_out]
+static int64_t head_wide_workspace_bytes(int64_t batch, int64_t dim, int64_t members) {
+  const int64_t n_out = 1 + dim + members * dim;
+  return align_up(2 * wide_geom(batch, dim, members).cta_cap * n_out * (int64_t)sizeof(float), 256);
+}
+static size_t head_wide_smem_bytes(int64_t dim) {
+  const WideGeom g = wide_geom(1, dim, 1);
+  return ((size_t)g.rb * g.ld + (size_t)g.rb * kMaxMembers + kWThreads / 32) * sizeof(float);
+}
+
 static void launch_head_group(const HeadGroup& g, int n_cta, size_t smem, cudaStream_t st) {
   const dim3 grid((unsigned)n_cta, (unsigned)g.n);
   switch (g.p[0].dim) {    // every op of a call shares dim
@@ -433,6 +726,7 @@ int heads_init() {
   ADN_HEAD_ATTR(0); ADN_HEAD_ATTR(1); ADN_HEAD_ATTR(2); ADN_HEAD_ATTR(3); ADN_HEAD_ATTR(4); ADN_HEAD_ATTR(10);
   ADN_HEAD_ATTR(16);
 #undef ADN_HEAD_ATTR
+  ADN_CUDA(cudaFuncSetAttribute(ensemble_head_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
   return ADN_OK;
 }
 
@@ -440,9 +734,13 @@ int64_t head_workspace_bytes_public(int64_t batch, int64_t dim, int64_t members)
   return head_workspace_bytes(batch, dim, members < 1 ? 1 : members);
 }
 
+int64_t head_wide_workspace_bytes_public(int64_t batch, int64_t dim, int64_t members) {
+  return head_wide_workspace_bytes(batch < 1 ? 1 : batch, dim < 1 ? 1 : dim, members < 1 ? 1 : members);
+}
+
 // Checks one op (`what` names it in messages) and fills its launch parameters; touches no device memory.
 static int head_group_op(const adn_head_op& o, const char* what, int64_t batch, int64_t dim, int fmt, int n_cta,
-                         HeadParams& p) {
+                         bool wide, HeadParams& p) {
   if (!o.members_host || !o.out3 || !o.workspace) return fail(ADN_ERR_INVALID, "%s: null pointer", what);
   if (o.head < 0 || o.head > 2 || o.mixture_type < 0 || o.mixture_type > 2)
     return fail(ADN_ERR_INVALID, "%s: bad head / mixture type (%d, %d)", what, o.head, o.mixture_type);
@@ -484,29 +782,45 @@ static int head_group_op(const adn_head_op& o, const char* what, int64_t batch, 
   p.dbias = o.dbias;
   const int wdim = (p.mixture == ADN_MIX_SCALAR) ? 1 : p.dim;
   p.n_out = 1 + p.dim + p.n_members * wdim;
-  if (o.workspace_bytes < head_workspace_bytes(batch, dim, o.n_members))
-    return fail(ADN_ERR_WORKSPACE, "%s: workspace %lld < %lld bytes", what, (long long)o.workspace_bytes,
-                (long long)head_workspace_bytes(batch, dim, o.n_members));
+  const int64_t need = wide ? head_wide_workspace_bytes(batch, dim, o.n_members) : head_workspace_bytes(batch, dim, o.n_members);
+  if (o.workspace_bytes < need)
+    return fail(ADN_ERR_WORKSPACE, "%s: workspace %lld < %lld bytes", what, (long long)o.workspace_bytes, (long long)need);
   p.part = reinterpret_cast<float*>(o.workspace);
   p.n_cta = n_cta;
+  if (wide) {
+    const WideGeom g = wide_geom(batch, dim, o.n_members);
+    p.n_cta = g.n_cta;
+    p.rb = g.rb;
+    p.bpc = g.bpc;
+    p.ld = g.ld;
+    // 16 B loads and stores of every row the kernel streams, when all of them are 16 B aligned
+    bool al = dim % 4 == 0;
+    auto a16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
+    for (int k = 0; k < o.n_members; ++k) al = al && a16(o.members_host[k]);
+    if (o.head != ADN_HEAD_SOFTMAX_XENT) al = al && a16(o.labels_f);
+    if (o.mixture_type == ADN_MIX_VECTOR && o.w) al = al && a16(o.w);
+    if (o.dens) al = al && a16(o.dens);
+    if (o.ens_out) al = al && a16(o.ens_out);
+    p.vec = al ? 1 : 0;
+  }
   return ADN_OK;
 }
 
 // Fills the launch of ops [i0, i0 + m) and the shared memory it needs.  A grouped call (`per_op`) names each op by
 // its index after `what`.
 static int head_group_chunk(const adn_head_op* ops, int i0, int m, int64_t batch, int64_t dim, int fmt, int n_cta,
-                            const char* what, bool per_op, HeadGroup& g, size_t& smem) {
+                            const char* what, bool per_op, bool wide, HeadGroup& g, size_t& smem) {
   g = HeadGroup{};
   g.n = m;
   smem = 0;
   for (int i = 0; i < m; ++i) {
     char name[64];
     if (per_op) snprintf(name, sizeof(name), "%s: op %d", what, i0 + i);
-    const int rc = head_group_op(ops[i0 + i], per_op ? name : what, batch, dim, fmt, n_cta, g.p[i]);
+    const int rc = head_group_op(ops[i0 + i], per_op ? name : what, batch, dim, fmt, n_cta, wide, g.p[i]);
     if (rc) return rc;
-    smem = std::max(smem, head_smem_bytes(g.p[i].dim, g.p[i].n_members));
+    smem = std::max(smem, wide ? head_wide_smem_bytes(dim) : head_smem_bytes(g.p[i].dim, g.p[i].n_members));
   }
-  if (smem > 227 * 1024) return fail(ADN_ERR_UNSUPPORTED, "%s: members x dim does not fit shared memory", what);
+  if (!wide && smem > kHeadSmemMax) return fail(ADN_ERR_UNSUPPORTED, "%s: members x dim does not fit shared memory", what);
   return ADN_OK;
 }
 
@@ -523,11 +837,12 @@ static int run_heads(const adn_head_op* ops, int n, int64_t batch, int64_t dim, 
   size_t smem;
   int rc;
   for (int i0 = 0; i0 < n; i0 += kMaxGroup)
-    if ((rc = head_group_chunk(ops, i0, std::min(kMaxGroup, n - i0), batch, dim, fmt, n_cta, what, per_op, g, smem)))
+    if ((rc = head_group_chunk(ops, i0, std::min(kMaxGroup, n - i0), batch, dim, fmt, n_cta, what, per_op, false, g,
+                               smem)))
       return rc;
   for (int i0 = 0; i0 < n; i0 += kMaxGroup) {
     const int m = std::min(kMaxGroup, n - i0);
-    if ((rc = head_group_chunk(ops, i0, m, batch, dim, fmt, n_cta, what, per_op, g, smem))) return rc;
+    if ((rc = head_group_chunk(ops, i0, m, batch, dim, fmt, n_cta, what, per_op, false, g, smem))) return rc;
     if (n_cta <= 512) {
       launch_head_group(g, n_cta, smem, st);
       ADN_CHECK_LAUNCH("ensemble_head_group");
@@ -551,6 +866,34 @@ static int run_heads(const adn_head_op* ops, int n, int64_t batch, int64_t dim, 
       ensemble_finalize_group_kernel<<<1, 256, 0, st>>>(one);
       ADN_CHECK_LAUNCH("ensemble_finalize_group");
     }
+  }
+  return ADN_OK;
+}
+
+// adn_head_group_wide: the same ops, validation and partials as run_heads, on the wide kernel (no shared-memory fit,
+// dim up to kWMaxDim).  At most kWMaxCta CTAs per op, so one head launch and one finalize launch per kMaxGroup ops.
+static int run_heads_wide(const adn_head_op* ops, int n, int64_t batch, int64_t dim, cudaStream_t st) {
+  const char* what = "adn_head_group_wide";
+  if (n < 0 || (n > 0 && !ops)) return fail(ADN_ERR_INVALID, "%s: bad ops", what);
+  if (batch <= 0) return fail(ADN_ERR_INVALID, "%s: bad batch %lld", what, (long long)batch);
+  if (dim < 1 || dim > kWMaxDim)
+    return fail(ADN_ERR_UNSUPPORTED, "%s: dim %lld not in [1,%d]", what, (long long)dim, kWMaxDim);
+  const int fmt = pl::format();
+  HeadGroup g;
+  size_t smem;
+  int rc;
+  for (int i0 = 0; i0 < n; i0 += kMaxGroup)
+    if ((rc = head_group_chunk(ops, i0, std::min(kMaxGroup, n - i0), batch, dim, fmt, 0, what, true, true, g, smem)))
+      return rc;
+  for (int i0 = 0; i0 < n; i0 += kMaxGroup) {
+    const int m = std::min(kMaxGroup, n - i0);
+    if ((rc = head_group_chunk(ops, i0, m, batch, dim, fmt, 0, what, true, true, g, smem))) return rc;
+    int n_cta = 1;
+    for (int i = 0; i < m; ++i) n_cta = std::max(n_cta, g.p[i].n_cta);
+    ensemble_head_wide_kernel<<<dim3((unsigned)n_cta, (unsigned)m), kWThreads, smem, st>>>(g);
+    ADN_CHECK_LAUNCH("ensemble_head_wide");
+    ensemble_finalize_group_kernel<<<m, 256, 0, st>>>(g);
+    ADN_CHECK_LAUNCH("ensemble_finalize_group");
   }
   return ADN_OK;
 }
@@ -632,6 +975,10 @@ extern "C" int adn_ensemble_head(int head, int mixture_type, const float* const*
 extern "C" int adn_head_group(const adn_head_op* ops, int n, int64_t batch, int64_t dim, void* stream) {
   if (n < 0 || (n > 0 && !ops)) return fail(ADN_ERR_INVALID, "adn_head_group: bad ops");
   return run_heads(ops, n, batch, dim, "adn_head_group", true, as_stream(stream));
+}
+
+extern "C" int adn_head_group_wide(const adn_head_op* ops, int n, int64_t batch, int64_t dim, void* stream) {
+  return run_heads_wide(ops, n, batch, dim, as_stream(stream));
 }
 
 extern "C" int adn_ema_update(float* state, const float* loss, float decay, void* stream) {

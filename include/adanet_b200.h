@@ -87,6 +87,8 @@ extern "C" {
 #define ADN_Q_PLANE_FORMAT 12             /* current ADN_PLANES_* */
 #define ADN_Q_TMA_MAP_CACHE_HITS 13       /* TMA descriptor cache statistics */
 #define ADN_Q_TMA_MAP_CACHE_MISSES 14
+#define ADN_Q_HEAD_PATH 15                /* a=dim b=members -> 0: adn_head_group, 1: adn_head_group_wide */
+#define ADN_Q_HEAD_WIDE_WORKSPACE_BYTES 16 /* a=batch b=dim c=members (adn_head_group_wide) */
 
 const char* adn_last_error(void);
 /* One-time, idempotent host-side initialisation (kernel attributes, driver entry
@@ -349,6 +351,12 @@ typedef struct adn_head_op {
   int64_t workspace_bytes;
 } adn_head_op;
 int adn_head_group(const adn_head_op* ops_host, int n, int64_t batch, int64_t dim, void* stream);
+/* adn_head_group for heads of any width: the same ops, outputs and checks, on a kernel that keeps no shared-memory
+ * copy of the members, so neither dim <= 64 nor the members x dim fit applies.  dim 1..16384 and n_members 1..64,
+ * anything else is ADN_ERR_UNSUPPORTED; each op's workspace is adn_query(ADN_Q_HEAD_WIDE_WORKSPACE_BYTES, batch, dim,
+ * n_members) instead.  adn_query(ADN_Q_HEAD_PATH, dim, n_members) says which of the two an op runs on.  Every
+ * reduction runs in an order fixed by (batch, dim, n_members).  One head launch and one finalize launch per 24 ops. */
+int adn_head_group_wide(const adn_head_op* ops_host, int n, int64_t batch, int64_t dim, void* stream);
 /* Per-step bookkeeping of n candidate ensembles in one launch: state <- zero-debiased EMA of out3[2] (adn_ema_update)
  * and trace[(*step_dev % capacity)][0..3] = {*sub_loss, out3[0], out3[2], ema} (adn_record_scalars).  Every entry is
  * checked before anything is launched: a call that returns an error has written nothing. */
