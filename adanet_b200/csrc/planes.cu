@@ -202,13 +202,15 @@ struct Item {
 // warps of a CTA decodes every work item, and on the thin-K layer waves that was a quarter of the stall samples.)
 __device__ __forceinline__ int fast_div(int n, float inv) { return (int)(((float)n + 0.5f) * inv); }
 
+// TBN: the tile width (columns) the problem's tiles_n counts
+template <int TBN = BN>
 __device__ __forceinline__ Item decode_item(const GemmParams& g, int item) {
   Item it;
   it.split = (g.splits == 1) ? 0 : fast_div(item, g.inv_tiles);
   const int t = item - it.split * g.tiles;
   const int tm = (g.tiles_n == 1) ? t : fast_div(t, g.inv_tiles_n);
   it.m0 = tm * BM;
-  it.n0 = (t - tm * g.tiles_n) * BN;
+  it.n0 = (t - tm * g.tiles_n) * TBN;
   it.kb0 = it.split * g.kb_per_split;
   it.nkb = min(g.total_kb, it.kb0 + g.kb_per_split) - it.kb0;
   return it;
@@ -585,36 +587,46 @@ __device__ __forceinline__ int acc_off(int row, int col) {
 }
 
 // adds one 128-K chunk of the MMA accumulators into the register accumulator with fp32 RN
-template <int FMT>
-__device__ __forceinline__ void fold_chunk(float (&acc)[32], const float (&H)[32], const float (&S)[32]) {
+template <int FMT, int R>
+__device__ __forceinline__ void fold_chunk(float (&acc)[R], const float (&H)[R], const float (&S)[R]) {
 #pragma unroll
-  for (int j = 0; j < 32; ++j) acc[j] += H[j];
+  for (int j = 0; j < R; ++j) acc[j] += H[j];
   if (FMT == FMT_F16) {
 #pragma unroll
-    for (int j = 0; j < 32; ++j) acc[j] = fmaf(S[j], 1.0f / 2048.0f, acc[j]);   // lo' carries 2^11
+    for (int j = 0; j < R; ++j) acc[j] = fmaf(S[j], 1.0f / 2048.0f, acc[j]);   // lo' carries 2^11
   } else {
 #pragma unroll
-    for (int j = 0; j < 32; ++j) acc[j] += S[j];
+    for (int j = 0; j < R; ++j) acc[j] += S[j];
   }
 }
 
 // One k-block of a consumer warpgroup on fp16 planes: 4 K steps of 16, each hi*hi into H and hi*lo' + lo'*hi into S
 // (first: the chunk starts, the MMAs overwrite H and S).  The warpgroup's 64 A rows start 8 KiB into the A tiles in
 // both majornesses; a K step advances 32 B inside a K-major 128 B row, 16 rows of 128 B in an MN-major tile.
-// a_hi: the warpgroup's 64 rows of the A hi tile, with the lo' tile A_TILE after it; b_hi: the B hi tile, with the
-// lo' tile B_TILE after it.
-template <int A_MN, int B_MN>
-__device__ __forceinline__ void f16_kblock_at(uint32_t a_hi, uint32_t b_hi, float (&H)[32], float (&S)[32], bool first) {
-  const uint32_t a_lo = a_hi + A_TILE, b_lo = b_hi + B_TILE;
+// a_hi: the warpgroup's 64 rows of the A hi tile, with the lo' tile A_TILE after it; b_hi: the B hi tile of TBN
+// columns, with the lo' tile TBN * 128 B after it.  An MN-major B tile of 128 columns is two [64 k][64 n] swizzle
+// atoms 8 KiB apart, its descriptor's leading byte offset.
+template <int A_MN, int B_MN, int TBN = BN>
+__device__ __forceinline__ void f16_kblock_at(uint32_t a_hi, uint32_t b_hi, float (&H)[TBN / 2], float (&S)[TBN / 2],
+                                              bool first) {
+  static_assert(TBN == 64 || TBN == 128, "tile width");
+  const uint32_t a_lo = a_hi + A_TILE, b_lo = b_hi + TBN * 128;
   constexpr uint32_t a_step = A_MN ? 2048u : 32u, b_step = B_MN ? 2048u : 32u;
+  constexpr uint32_t b_lbo = (B_MN && TBN == 128) ? 8192u : 1024u;
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
     const uint32_t sd = (first && k == 0) ? 0u : 1u;
     const uint64_t dah = wg::desc_sw128(a_hi + k * a_step), dal = wg::desc_sw128(a_lo + k * a_step);
-    const uint64_t dbh = wg::desc_sw128(b_hi + k * b_step), dbl = wg::desc_sw128(b_lo + k * b_step);
-    wg::mma_f16_n64<A_MN, B_MN>(H, dah, dbh, sd);
-    wg::mma_f16_n64<A_MN, B_MN>(S, dah, dbl, sd);
-    wg::mma_f16_n64<A_MN, B_MN>(S, dal, dbh, 1u);
+    const uint64_t dbh = wg::desc_sw128(b_hi + k * b_step, b_lbo), dbl = wg::desc_sw128(b_lo + k * b_step, b_lbo);
+    if constexpr (TBN == 64) {
+      wg::mma_f16_n64<A_MN, B_MN>(H, dah, dbh, sd);
+      wg::mma_f16_n64<A_MN, B_MN>(S, dah, dbl, sd);
+      wg::mma_f16_n64<A_MN, B_MN>(S, dal, dbh, 1u);
+    } else {
+      wg::mma_f16_n128<A_MN, B_MN>(H, dah, dbh, sd);
+      wg::mma_f16_n128<A_MN, B_MN>(S, dah, dbl, sd);
+      wg::mma_f16_n128<A_MN, B_MN>(S, dal, dbh, 1u);
+    }
   }
 }
 // the same on one pipeline stage of pl_gemm_kernel (A_hi A_lo B_hi B_lo)
@@ -888,6 +900,149 @@ template <int FMT>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 pl_gemm_ms_kernel(const __grid_constant__ MsGroup grp) {
   pl_gemm_body<FMT, EPI_BIAS_ACT>(grp);
+}
+
+// ---------------------------------------------------------------------------------
+// Wide dW kernel (pl_dw_kernel): the fp16 dW waves (EPI_PARTIAL) on 128 x 128 tiles.  pl_gemm_kernel's 128 x 64 tile
+// issues m64n64k16, whose 4 KiB of operands per 65,536 MACs take all of an SM's shared-memory bandwidth at the tensor
+// rate, and re-reads its A rows from L2 once per 64 output columns.  Here each consumer warpgroup owns 64 rows x 128
+// columns and issues m64n128k16 (6 KiB per 131,072 MACs), and A is read once per 128 columns.  A dW work item ends in
+// a plain fp32 store of its tile (the split-K partial, or dW itself with one split), so there is no epilogue
+// warpgroup: the consumers store their fragments straight from registers while the producer refills the ring, and the
+// register file goes to the three accumulators of 64 x 128 outputs (H, S and the RN-folded acc, 64 each).
+// Work items, split boundaries and the per-element arithmetic (bias-free start, f16_kblock_at, fold_chunk every 128 K,
+// out_mul) are pl_gemm_kernel's, so dW is bit-identical to it.  One thread of the producer warpgroup issues the TMA
+// loads: A_hi, A_lo', B_hi, B_lo' as MN-major [2][64 k][64 mn] boxes of 16 KiB each per k-block.
+// ---------------------------------------------------------------------------------
+static constexpr int DW_BN = 128;
+static constexpr int DW_B_TILE = DW_BN * 128;                  // 16 KiB
+static constexpr int DW_STAGE_BYTES = 2 * A_TILE + 2 * DW_B_TILE;   // A_hi A_lo B_hi B_lo: 64 KiB
+static constexpr int DW_THREADS = 128 * (1 + CONSUMERS);
+static constexpr int DW_CONSUMER_REGS = 232;
+static_assert(128 * PRODUCER_REGS + 128 * CONSUMERS * DW_CONSUMER_REGS <= 65536, "register file");
+static_assert(PRODUCER_REGS < 65536 / DW_THREADS && DW_CONSUMER_REGS > 65536 / DW_THREADS, "setmaxnreg.dec / .inc");
+static constexpr int DW_SMEM_BYTES = 1024 + STAGES * DW_STAGE_BYTES + BAR_BYTES;
+static_assert(DW_SMEM_BYTES <= 232448, "shared memory per block");
+
+__global__ void __launch_bounds__(DW_THREADS, 1)
+pl_dw_kernel(const __grid_constant__ Group grp) {
+  constexpr int BK = Fmt<FMT_F16>::BK;
+  constexpr int CHUNK = Fmt<FMT_F16>::CHUNK;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * DW_STAGE_BYTES);
+  uint64_t* full_bar = bars;                       // [STAGES]  TMA -> consumers
+  uint64_t* empty_bar = bars + STAGES;             // [STAGES]  consumers -> TMA, count CONSUMER_WARPS
+
+  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
+  const int lane = threadIdx.x & 31;
+  const int n_items = grp.total_items;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(smem_u32(&full_bar[s]), 1);
+      mbar_init(smem_u32(&empty_bar[s]), CONSUMER_WARPS);
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  if (warp == 1 && lane < grp.n) {
+    tma_prefetch_desc(&grp.p[lane].a_hi);
+    tma_prefetch_desc(&grp.p[lane].a_lo);
+    tma_prefetch_desc(&grp.p[lane].b_hi);
+    tma_prefetch_desc(&grp.p[lane].b_lo);
+  }
+  __syncthreads();
+
+  if (warp < 4) {
+    // ================= TMA producer =================
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (warp == 0 && lane == 0) {
+      uint32_t s = 0, ph = 0;
+      int cur = 0, next0 = first_next0(grp);
+      const uint32_t smem0 = smem_u32(smem);
+      for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+        cur = find_problem(grp, cur, item, next0);
+        const Problem& pr = grp.p[cur];
+        const Item it = decode_item<DW_BN>(pr.g, item - pr.item0);
+        for (int kb = 0; kb < it.nkb; ++kb) {
+          mbar_wait(smem_u32(&empty_bar[s]), ph ^ 1);
+          const uint32_t fb = smem_u32(&full_bar[s]);
+          mbar_expect_tx(fb, DW_STAGE_BYTES);
+          const uint32_t base = smem0 + s * DW_STAGE_BYTES;
+          const int kc = it.kb0 + kb;
+          // MN-major boxes {BK, BK k-rows, 2 blocks of 64 columns} at (0, kc * BK, mn0 / BK)
+          tma_load_3d(&pr.a_hi, fb, base, 0, kc * BK, it.m0 / BK);
+          tma_load_3d(&pr.a_lo, fb, base + A_TILE, 0, kc * BK, it.m0 / BK);
+          tma_load_3d(&pr.b_hi, fb, base + 2 * A_TILE, 0, kc * BK, it.n0 / BK);
+          tma_load_3d(&pr.b_lo, fb, base + 2 * A_TILE + DW_B_TILE, 0, kc * BK, it.n0 / BK);
+          if (++s == STAGES) { s = 0; ph ^= 1; }
+        }
+      }
+    }
+    return;
+  }
+
+  // ================= consumer warpgroups 1..2 =================
+  setmaxnreg_inc<DW_CONSUMER_REGS>();
+  const int wgi = warp / 4 - 1;                    // which 64 rows of the tile
+  const int wq = warp & 3;
+  const int gid = lane >> 2, tq = lane & 3;        // accumulator fragment coordinates
+  const uint32_t smem0 = smem_u32(smem);
+  uint32_t s = 0, ph = 0;
+  int cur = 0, next0 = first_next0(grp);
+  float H[64], S[64];                              // MMA accumulators of one 128-K chunk
+#pragma unroll
+  for (int j = 0; j < 64; ++j) H[j] = S[j] = 0.f;
+  for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+    cur = find_problem(grp, cur, item, next0);
+    const GemmParams& g = grp.p[cur].g;
+    const Item it = decode_item<DW_BN>(g, item - grp.p[cur].item0);
+    float acc[64];
+#pragma unroll
+    for (int j = 0; j < 64; ++j) acc[j] = 0.f;
+    for (int kb = 0; kb < it.nkb; ++kb) {
+      const bool first = (kb % CHUNK) == 0;
+      const bool last = (kb % CHUNK) == CHUNK - 1 || kb == it.nkb - 1;
+      mbar_wait(smem_u32(&full_bar[s]), ph);
+      wg::fence_regs(H);
+      wg::fence_regs(S);
+      wg::fence();
+      const uint32_t st = smem0 + s * DW_STAGE_BYTES;
+      f16_kblock_at<1, 1, DW_BN>(st + (uint32_t)wgi * 8192u, st + 2 * A_TILE, H, S, first);
+      wg::commit();
+      wg::wait<0>();
+      wg::fence_regs(H);
+      wg::fence_regs(S);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(smem_u32(&empty_bar[s]));     // this warp is done with the stage
+      if (++s == STAGES) { s = 0; ph ^= 1; }
+      if (last) fold_chunk<FMT_F16>(acc, H, S);
+    }
+    // ---- the tile leaves from the fragment layout: a quad holds 8 consecutive columns (one 32 B sector) of a row ----
+    float* dense = reinterpret_cast<float*>(g.out) + (size_t)it.split * g.M * g.N;
+    const bool vec = (g.ldc & 1) == 0 && (reinterpret_cast<uintptr_t>(dense) & 7) == 0;
+    if (g.out_mul != 1.0f) {
+#pragma unroll
+      for (int j = 0; j < 64; ++j) acc[j] *= g.out_mul;
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = it.m0 + 64 * wgi + 16 * wq + gid + 8 * h;
+      if (row >= g.M) continue;
+      float* rp = dense + (size_t)row * g.ldc;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int col = it.n0 + 8 * j + 2 * tq;
+        const float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+        if (vec && col + 1 < g.N) {
+          *reinterpret_cast<float2*>(rp + col) = make_float2(v0, v1);
+        } else {
+          if (col < g.N) rp[col] = v0;
+          if (col + 1 < g.N) rp[col + 1] = v1;
+        }
+      }
+    }
+  }
 }
 
 // ---------------------------------------------------------------------------------
@@ -1240,6 +1395,7 @@ int init() {
     ok = ok && cudaFuncSetAttribute(pl_gemm_ms_kernel<FMT_F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) == cudaSuccess;
     ok = ok && cudaFuncSetAttribute(pl_thin_kernel<EPI_BIAS_ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, THIN_SMEM_BYTES) == cudaSuccess;
     ok = ok && cudaFuncSetAttribute(pl_thin_kernel<EPI_MASK>, cudaFuncAttributeMaxDynamicSharedMemorySize, THIN_SMEM_BYTES) == cudaSuccess;
+    ok = ok && cudaFuncSetAttribute(pl_dw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DW_SMEM_BYTES) == cudaSuccess;
     if (!ok) {
       (void)cudaGetLastError();
       rc = fail(ADN_ERR_CUDA, "pl::init: cudaFuncSetAttribute(smem=%d) failed", SMEM_BYTES);
@@ -1366,15 +1522,16 @@ struct GemmDesc {
   Operand sa[MAX_SRCS], sb[MAX_SRCS];
 };
 
+// bn: the B tile extent (columns of the result)
 static int encode_maps(int fmt, const GemmDesc& d, CUtensorMap* a_hi, CUtensorMap* a_lo, CUtensorMap* b_hi, CUtensorMap* b_lo,
-                       const char* what) {
+                       const char* what, int bn = BN) {
   if (!planes_aligned(d.a.hi) || !planes_aligned(d.a.lo) || !planes_aligned(d.b.hi) || !planes_aligned(d.b.lo))
     return fail(ADN_ERR_INVALID, "%s: plane buffers must be 256 B aligned", what);
   int rc;
   if ((rc = make_map(fmt, a_hi, d.a.hi, d.a.rows, d.a.nkb, d.a.mn_major, BM))) return rc;
   if ((rc = make_map(fmt, a_lo, d.a.lo, d.a.rows, d.a.nkb, d.a.mn_major, BM))) return rc;
-  if ((rc = make_map(fmt, b_hi, d.b.hi, d.b.rows, d.b.nkb, d.b.mn_major, BN))) return rc;
-  if ((rc = make_map(fmt, b_lo, d.b.lo, d.b.rows, d.b.nkb, d.b.mn_major, BN))) return rc;
+  if ((rc = make_map(fmt, b_hi, d.b.hi, d.b.rows, d.b.nkb, d.b.mn_major, bn))) return rc;
+  if ((rc = make_map(fmt, b_lo, d.b.lo, d.b.rows, d.b.nkb, d.b.mn_major, bn))) return rc;
   return ADN_OK;
 }
 
@@ -1386,6 +1543,26 @@ static bool thin_group(int fmt, const Group& grp) {
     if (!g.out_planes || g.splits != 1 || g.total_kb > Fmt<FMT_F16>::CHUNK) return false;
   }
   return true;
+}
+// A dW group (EPI_PARTIAL) runs on pl_dw_kernel when the format is fp16, padding every problem's N to 128 columns
+// instead of 64 adds at most 1/8 to the group's MMA work, and the wide items still spread over the SMs: work items are
+// dealt round-robin and a wide item is two narrow items of work, so the busiest SM may get at most one narrow item's
+// work more than with 128 x 64 tiles.  (The split plan is made for 128 x 64 tiles: the first-layer dW of the
+// benchmarked step has 135 wide items for 132 SMs, and three SMs doing two of them made that wave 37 % slower.)
+// Reads M, N, total_kb and splits only, which the tile does not change.
+static bool dw_group(int fmt, const Group& grp) {
+  if (fmt != FMT_F16) return false;
+  int64_t narrow = 0, wide = 0, items_n = 0, items_w = 0;
+  for (int i = 0; i < grp.n; ++i) {
+    const GemmParams& g = grp.p[i].g;
+    const int64_t tm = ceil_div(g.M, BM);
+    narrow += tm * g.total_kb * ceil_div(g.N, BN) * BN;
+    wide += tm * g.total_kb * ceil_div(g.N, DW_BN) * DW_BN;
+    items_n += tm * ceil_div(g.N, BN) * g.splits;
+    items_w += tm * ceil_div(g.N, DW_BN) * g.splits;
+  }
+  const int64_t sms = sm_count();
+  return 8 * wide <= 9 * narrow && 2 * ceil_div(items_w, sms) <= ceil_div(items_n, sms) + 1;
 }
 template <int FMT, int EPI>
 static void launch_kernel(const Group& grp, int grid, cudaStream_t st) {
@@ -1405,6 +1582,13 @@ static int build_groups(int fmt, const GemmDesc* d, int n, std::vector<G>& out, 
       out.emplace_back();
       G& grp = out.back();
       memset(&grp, 0, sizeof(grp));
+      // the tile width: 128 columns when the dW group goes to pl_dw_kernel (dw_group reads only the shapes set here)
+      int bn = BN;
+      if constexpr (!MS && EPI == EPI_PARTIAL) {
+        for (int i = 0; i < m; ++i) grp.p[i].g = d[i0 + i].g;
+        grp.n = m;
+        if (dw_group(fmt, grp)) bn = DW_BN;
+      }
       int items = 0;
       for (int i = 0; i < m; ++i) {
         const GemmDesc& src = d[i0 + i];
@@ -1412,7 +1596,7 @@ static int build_groups(int fmt, const GemmDesc* d, int n, std::vector<G>& out, 
         // the kernel fixes the operand majorness per epilogue kind (fwd: K / MN, dX: K / K, dW: MN / MN)
         if (src.a.mn_major != (EPI == EPI_PARTIAL) || src.b.mn_major != (EPI != EPI_MASK))
           return fail(ADN_ERR_INVALID, "%s: operand majorness does not match the epilogue kind", what);
-        int rc = encode_maps(fmt, src, &pr.a_hi, &pr.a_lo, &pr.b_hi, &pr.b_lo, what);
+        int rc = encode_maps(fmt, src, &pr.a_hi, &pr.a_lo, &pr.b_hi, &pr.b_lo, what, bn);
         if (rc) return rc;
         if constexpr (MS) {
           int kb = (int)src.a.nkb;
@@ -1437,7 +1621,7 @@ static int build_groups(int fmt, const GemmDesc* d, int n, std::vector<G>& out, 
         pr.g.a_mn = src.a.mn_major;
         pr.g.b_mn = src.b.mn_major;
         pr.g.tiles_m = (int)ceil_div(pr.g.M, BM);
-        pr.g.tiles_n = (int)ceil_div(pr.g.N, BN);
+        pr.g.tiles_n = (int)ceil_div(pr.g.N, bn);
         pr.g.tiles = pr.g.tiles_m * pr.g.tiles_n;
         if ((int64_t)pr.g.tiles * pr.g.splits >= (1 << 21))
           return fail(ADN_ERR_UNSUPPORTED, "%s: %d work items exceed the decode range", what, pr.g.tiles * pr.g.splits);
@@ -1476,6 +1660,8 @@ static int launch_groups(int fmt, const std::vector<G>& groups, cudaStream_t st,
       else pl_gemm_ms_kernel<FMT_TF32><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(grp);
     } else if (thin_group(fmt, grp)) {
       if constexpr (EPI != EPI_PARTIAL) pl_thin_kernel<EPI><<<grid, THIN_THREADS, THIN_SMEM_BYTES, st>>>(grp);
+    } else if (EPI == EPI_PARTIAL && dw_group(fmt, grp)) {
+      pl_dw_kernel<<<grid, DW_THREADS, DW_SMEM_BYTES, st>>>(grp);
     } else {
       if (fmt == FMT_F16) launch_kernel<FMT_F16, EPI>(grp, grid, st);
       else launch_kernel<FMT_TF32, EPI>(grp, grid, st);

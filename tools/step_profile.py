@@ -74,6 +74,8 @@ def classify(name):
   m = re.search(r"pl_thin_kernel<(\d+)>", name)
   if m:
     return "gemm", int(m.group(1))
+  if "pl_dw_kernel" in name:
+    return "gemm", 2
   for key, kind in (("reduce_partials", "reduce"), ("colsum", "colsum"), ("opt_step", "optimizer"),
                     ("step_increment", "optimizer"), ("split_kernel", "split"), ("head_bookkeeping", "bookkeeping"),
                     ("counter_add", "counter")):
