@@ -24,7 +24,10 @@ PATH_AUTO, PATH_SIMT, PATH_TCGEN05 = 0, 1, 2
 PLANES_TF32, PLANES_F16 = 0, 1
 (Q_VERSION, Q_DENSE_BWD_WS, Q_HEAD_WS, Q_DENSE_FWD_PATH, Q_SM_COUNT, Q_LAUNCH_COUNT, Q_DENSE_BWD_PATH,
  Q_DENSE_FWD_WS, Q_PLANES_BYTES, Q_DENSE_BWD_P_WS, Q_COLSUM_WS, Q_CONV_STEM_BWD_WS, Q_PLANE_FORMAT,
- Q_TMA_MAP_CACHE_HITS, Q_TMA_MAP_CACHE_MISSES, Q_HEAD_PATH, Q_HEAD_WIDE_WS) = range(17)
+ Q_TMA_MAP_CACHE_HITS, Q_TMA_MAP_CACHE_MISSES, Q_HEAD_PATH, Q_HEAD_WIDE_WS, Q_METRICS_WS) = range(18)
+METRICS_BINARY, METRICS_MEANS = 0, 1
+METRICS_THRESHOLDS = 200
+METRICS_COUNTS = 404  # 2 * (METRICS_THRESHOLDS + 1) + 2
 
 EXPORTS = (
     "adn_last_error", "adn_init", "adn_query", "adn_set_dense_path", "adn_dense_fwd", "adn_dense_bwd", "adn_head_loss",
@@ -33,7 +36,7 @@ EXPORTS = (
     "adn_opt_step_p", "adn_head_loss_p", "adn_dense_fwd_p_group", "adn_dense_bwd_p_group",
     "adn_l1_grad_add", "adn_conv_stem_fwd", "adn_conv_stem_bwd", "adn_set_plane_format", "adn_plane_overflow",
     "adn_planes_split_scaled", "adn_head_group", "adn_head_bookkeeping", "adn_opt_step_group",
-    "adn_head_group_wide",
+    "adn_head_group_wide", "adn_metrics_group",
 )
 
 
@@ -84,6 +87,12 @@ class OptOp(ctypes.Structure):
               ("grads_host", POINTER(c_void_p)), ("slot0_host", POINTER(c_void_p)), ("slot1_host", POINTER(c_void_p)),
               ("sizes_host", POINTER(c_int64)), ("hyper_host", POINTER(c_float)), ("step_dev", c_void_p),
               ("planes_host", POINTER(c_void_p)), ("cols_host", POINTER(c_int64))]
+
+
+class MetricsOp(ctypes.Structure):
+  """adn_metrics_op (include/adanet_b200.h)"""
+  _fields_ = [("kind", ctypes.c_int32), ("reserved", ctypes.c_int32), ("logits", c_void_p), ("labels_f", c_void_p),
+              ("dim", c_int64), ("counts", c_void_p), ("sums", c_void_p)]
 
 
 class AdnError(RuntimeError):
@@ -140,6 +149,7 @@ def load():
   lib.adn_head_group_wide.argtypes = [POINTER(HeadOp), c_int, i64, i64, p]
   lib.adn_head_bookkeeping.argtypes = [POINTER(HeadBook), c_int, p, p]
   lib.adn_opt_step_group.argtypes = [POINTER(OptOp), c_int, p]
+  lib.adn_metrics_group.argtypes = [POINTER(MetricsOp), c_int, i64, p, i64, p]
   for name in EXPORTS:
     if name != "adn_last_error":
       getattr(lib, name).restype = c_int

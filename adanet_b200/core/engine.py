@@ -45,6 +45,7 @@ import numpy as np
 import torch
 
 from adanet_b200 import _lib
+from adanet_b200.core import metrics as metrics_lib
 
 _HEAD_KIND = {"softmax_xent": _lib.HEAD_SOFTMAX_XENT, "mse": _lib.HEAD_MSE, "sigmoid_xent": _lib.HEAD_SIGMOID_XENT}
 _MIX_KIND = {"scalar": _lib.MIX_SCALAR, "vector": _lib.MIX_VECTOR, "matrix": _lib.MIX_MATRIX}
@@ -85,6 +86,53 @@ def _metric_value(metric: str, out3: torch.Tensor, ens_logits: Optional[torch.Te
   if metric == "accuracy":
     return accuracy_of(ens_logits[:b], labels[:b])
   return float(out3[2 if metric == "adanet_loss" else 0].item())
+
+
+class EnsembleMetrics:
+  """Streaming accumulators of the STREAM_METRICS (core/metrics.py) of n ensembles of one binary or regression head
+  kind: per ensemble an fp64 sums[3] and, for a binary head, the int64 threshold histograms and class-id counts of
+  adn_metrics_group, plus the persistent [batch, C] buffer its head writes the ensemble logits to.  `add` enqueues
+  one launch group over every ensemble; only `values` synchronises."""
+
+  def __init__(self, lib, head: str, n: int, batch: int, logits_dim: int, device,
+               ens_out: Optional[Sequence[torch.Tensor]] = None):
+    if head not in ("sigmoid_xent", "mse"):
+      raise ValueError("streaming metrics need a binary or regression head, not %s" % head)
+    self.lib, self.head, self.batch, self.C = lib, head, batch, logits_dim
+    self.kind = _lib.METRICS_BINARY if head == "sigmoid_xent" else _lib.METRICS_MEANS
+    self.ens_out = (list(ens_out) if ens_out is not None else
+                    [torch.empty((batch, logits_dim), dtype=torch.float32, device=device) for _ in range(n)])
+    self.counts = (torch.zeros((n, _lib.METRICS_COUNTS), dtype=torch.int64, device=device)
+                   if self.kind == _lib.METRICS_BINARY else None)
+    self.sums = torch.zeros((n, 3), dtype=torch.float64, device=device)
+    self.ws_bytes = _lib.query(_lib.Q_METRICS_WS, batch, logits_dim, n)
+    self.ws = torch.empty((self.ws_bytes,), dtype=torch.uint8, device=device)
+
+  def reset(self):
+    self.sums.zero_()
+    if self.counts is not None:
+      self.counts.zero_()
+
+  def add(self, labels_f: torch.Tensor, rows: int, sp: int):
+    """Adds the first `rows` rows of every ensemble's ens_out against `labels_f` to its accumulators (nothing on a rank
+    that owns no candidate ensemble)."""
+    n = len(self.ens_out)
+    if n == 0:
+      return
+    ops = (_lib.MetricsOp * n)(*[
+        _lib.MetricsOp(self.kind, 0, out.data_ptr(), labels_f.data_ptr(), self.C,
+                       self.counts[i].data_ptr() if self.counts is not None else None, self.sums[i].data_ptr())
+        for i, out in enumerate(self.ens_out)])
+    _lib.check(self.lib.adn_metrics_group(ops, n, rows, self.ws.data_ptr(), self.ws_bytes, sp), "adn_metrics_group")
+
+  def results(self) -> List[Dict[str, float]]:
+    """The finalized metric dict of every ensemble (one D2H read)."""
+    sums = self.sums.cpu().numpy()
+    counts = self.counts.cpu().numpy() if self.counts is not None else [None] * len(sums)
+    return [metrics_lib.finalize(c, s) for c, s in zip(counts, sums)]
+
+  def values(self, metric: str) -> List[float]:
+    return [r[metric] for r in self.results()]
 
 
 MAX_HEAD_DIM = 16384        # widest head adn_head_group_wide runs
@@ -1514,6 +1562,29 @@ class IterationPlan:
       h.enqueue_eval(self.labels, self.labels_f, ens_out, sp, self.xp, rows=b)
     return [_metric_value(metric, h.out3, ens_out, labels, b) for (_, h, _), ens_out in zip(self.heads, ens_outs)]
 
+  def stream_metrics(self, metric: str) -> EnsembleMetrics:
+    """Starts a streaming evaluation of a core/metrics.STREAM_METRICS `metric` (AUC, precision, recall, means) of
+    every local candidate ensemble: returns the zeroed accumulators that `stream_eval_step` adds each hold-out batch
+    to, one per head in `self.heads` order."""
+    metrics_lib.check_stream_metric(metric, self.head)
+    if self.sharded:
+      raise NotImplementedError("hold-out evaluation of row-sharded candidates: use placement='balanced' with an Evaluator")
+    if getattr(self, "_metrics", None) is None:
+      self._metrics = EnsembleMetrics(self.lib, self.head, len(self.heads), self.batch, self.C, self.device)
+    self._metrics.reset()
+    return self._metrics
+
+  def stream_eval_step(self, x, y):
+    """Adds one hold-out batch of b <= batch examples to the accumulators of `stream_metrics`: the members in inference
+    mode at the static batch (a partial batch zero-padded), every head's ensemble logits into its persistent buffer,
+    then one adn_metrics_group over the first b rows of every ensemble.  Nothing is read back."""
+    b = _load_rows(self.x, self.labels_f, x, y)
+    sp = torch.cuda.current_stream(self.device).cuda_stream
+    _forward_inference(self.lib, list(self.frozen) + [c.net for c in self.candidates], self.x, self.xp, sp)
+    for (_, h, _), ens_out in zip(self.heads, self._metrics.ens_out):
+      h.enqueue_eval(self.labels, self.labels_f, ens_out, sp, self.xp, rows=b)
+    self._metrics.add(self.labels_f, b, sp)
+
   # -- in-flight checkpoint -------------------------------------------------------
   def state_dict(self) -> Dict[str, np.ndarray]:
     """State of the iteration in flight on this GPU (one flat dict, keys prefixed by candidate index)."""
@@ -1587,7 +1658,7 @@ class EnsembleEvalPlan:
     """`mix_w`: the SCALAR [N] / VECTOR [N, C] mixture weights, or the list of the N MATRIX W_k [D_k, C]."""
     self.lib = _require_cuda()
     self.device = device or torch.device("cuda", torch.cuda.current_device())
-    self.batch, self.C = batch, logits_dim
+    self.batch, self.C, self.head_kind = batch, logits_dim, head
     self.fmt = _lib.plane_format()      # xp and the head's planes are sized for it: a plan outlives no format switch
     for m in members:
       m.ensure_format()
@@ -1620,12 +1691,35 @@ class EnsembleEvalPlan:
     """Evaluates the ensemble on the b <= batch examples of `x`: returns (loss, reg, adanet_loss) over them as
     floats (NaN-free only when labels given) and leaves their ensemble logits in the first b rows of
     `self.ens_logits` (`self.rows` = b).  The members run at the static batch, a partial batch zero-padded."""
+    self._enqueue_run(x, y)
+    o = self.out3.cpu().numpy()
+    return float(o[0]), float(o[1]), float(o[2])
+
+  def _enqueue_run(self, x, y):
     sp = torch.cuda.current_stream(self.device).cuda_stream
     self.rows = _load_rows(self.x, self.labels if self.labels is not None else self.labels_f, x, y)
     _forward_inference(self.lib, self.head.member_nets, self.x, self.xp, sp)
     self.head.enqueue_eval(self.labels, self.labels_f, self.ens_logits, sp, self.xp, rows=self.rows)
-    o = self.out3.cpu().numpy()
-    return float(o[0]), float(o[1]), float(o[2])
+    return sp
+
+  def stream_metrics(self, metric: Optional[str] = None) -> EnsembleMetrics:
+    """Zeroed streaming accumulators over this ensemble's logits buffer (IterationPlan.stream_metrics); `metric`, if
+    given, is checked against the head first."""
+    if metric is not None:
+      metrics_lib.check_stream_metric(metric, self.head_kind)
+    if getattr(self, "_metrics", None) is None:
+      self._metrics = EnsembleMetrics(self.lib, self.head_kind, 1, self.batch, self.C, self.device, [self.ens_logits])
+    self._metrics.reset()
+    return self._metrics
+
+  def add_metrics(self):
+    """Adds the examples of the last `run` to the accumulators of `stream_metrics`."""
+    self._metrics.add(self.labels_f, self.rows, torch.cuda.current_stream(self.device).cuda_stream)
+
+  def stream_eval_step(self, x, y):
+    """Evaluates the ensemble on a batch and adds it to the accumulators of `stream_metrics`, reading nothing back."""
+    self._enqueue_run(x, y)
+    self.add_metrics()
 
   def metric(self, x, y, metric: str = "adanet_loss") -> float:
     """One Evaluator metric of the finished ensemble on a batch (see IterationPlan.eval_step)."""

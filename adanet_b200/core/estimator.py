@@ -29,6 +29,7 @@ from adanet_b200 import graph
 from adanet_b200 import train as train_lib
 from adanet_b200.core import input_utils
 from adanet_b200.core.architecture import _Architecture
+from adanet_b200.core.metrics import STREAM_METRICS
 
 
 class RunConfig:
@@ -642,7 +643,20 @@ class Estimator(object):
         os.remove(self._inflight_path())
       return None
     builders, subs = self._pending
-    if self._evaluator is not None:
+    if self._evaluator is not None and self._evaluator.metric_name in STREAM_METRICS:
+      ev, name = self._evaluator, self._evaluator.metric_name
+      to_x = lambda f: input_utils.to_matrix(f, self._feature_keys)
+      prev_metric = None
+      if t > 0:
+        plan_prev = self._ensemble_eval_plan()
+        acc = plan_prev.stream_metrics(name)
+        prev_metric = ev.evaluate_streaming(lambda f, l: plan_prev.stream_eval_step(to_x(f), l),
+                                            lambda: acc.values(name))[0]
+      def local_metric(plan):
+        acc = plan.stream_metrics(name)
+        return ev.evaluate_streaming(lambda f, l: plan.stream_eval_step(to_x(f), l), lambda: acc.values(name))
+      rep = s.finish_iteration(local_metric_fn=local_metric, previous_metric=prev_metric, objective_fn=ev.objective_fn)
+    elif self._evaluator is not None:
       ev = self._evaluator
       prev_metric = None
       if t > 0:
@@ -786,11 +800,15 @@ class Estimator(object):
     """Metrics of the best ensemble over `steps` batches of at most the training batch size, a partial last batch
     included: `loss` (the mean of the per-batch mean losses), `average_loss` (the mean over examples), `accuracy`
     for classification heads (over examples), `global_step`, `iteration` and the architecture string
-    (eval_metrics.py:120,227-264,347-393)."""
+    (eval_metrics.py:120,227-264,347-393); a BinaryClassHead adds `precision`, `recall`, `auc`,
+    `auc_precision_recall`, `prediction/mean`, `label/mean` and `accuracy_baseline`, a RegressionHead
+    `prediction/mean` and `label/mean` (the v2 heads' metrics, streamed over every batch: core/metrics.py)."""
     import torch
     from adanet_b200.core import engine as eng
     self._restore_for_inference(input_fn)
     plan = self._ensemble_eval_plan()
+    streams = self._head.loss_kind in ("sigmoid_xent", "mse")
+    acc = plan.stream_metrics() if streams else None
     n, loss_sum, examples, example_loss_sum, correct, total = 0, 0.0, 0, 0.0, 0, 0
     for features, labels in input_utils.iterate_input_fn(input_fn):
       if steps is not None and n >= steps:
@@ -801,6 +819,8 @@ class Estimator(object):
       n += 1
       example_loss_sum += loss * b
       examples += b
+      if streams:
+        plan.add_metrics()
       if self._head.loss_kind != "mse":
         c, t = eng.correct_of(plan.ens_logits[:b], torch.as_tensor(labels).to(plan.device))
         correct += c
@@ -811,6 +831,8 @@ class Estimator(object):
            "iteration": self._search.iteration, "architecture/adanet/ensembles": self.architecture_string()}
     if total:
       out["accuracy"] = correct / total
+    if streams:
+      out.update(acc.results()[0])
     return out
 
   def predict(self, input_fn, predict_keys=None, hooks=None, checkpoint_path=None, yield_single_examples=True):

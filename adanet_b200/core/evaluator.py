@@ -59,3 +59,19 @@ class Evaluator(object):
     if n == 0:
       raise ValueError("Evaluator input_fn produced no batches")
     return list(sums / weight)
+
+  def evaluate_streaming(self, add_batch_fn, values_fn):
+    """The metrics that are not means of per-batch values (auc, precision, recall, ...: core/metrics.STREAM_METRICS):
+    streams up to `steps` batches of `input_fn` through `add_batch_fn(features, labels)`, which adds each to the
+    candidates' confusion counts and sums, then returns `values_fn()`, one finalized value per candidate (the
+    streaming Keras metrics of evaluator.py:97-140)."""
+    from adanet_b200.core.input_utils import iterate_input_fn
+    n = 0
+    for features, labels in iterate_input_fn(self._input_fn):
+      if self._steps is not None and n == self._steps:
+        break
+      add_batch_fn(features, labels)
+      n += 1
+    if n == 0:
+      raise ValueError("Evaluator input_fn produced no batches")
+    return list(values_fn())

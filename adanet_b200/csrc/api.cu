@@ -56,6 +56,7 @@ int64_t head_workspace_bytes_public(int64_t batch, int64_t dim, int64_t members)
 int64_t head_wide_workspace_bytes_public(int64_t batch, int64_t dim, int64_t members);
 int head_path(int64_t dim, int64_t members);
 int heads_init();
+namespace metrics { int64_t workspace_bytes(int64_t rows, int64_t dim, int64_t n); }
 
 }  // namespace adn
 
@@ -114,6 +115,7 @@ extern "C" int adn_query(int key, int64_t a, int64_t b, int64_t c, int64_t* out_
     case ADN_Q_HEAD_WORKSPACE_BYTES: *out_host = head_workspace_bytes_public(a, b, c) + 256; return ADN_OK;
     case ADN_Q_HEAD_PATH: *out_host = head_path(a, b); return ADN_OK;
     case ADN_Q_HEAD_WIDE_WORKSPACE_BYTES: *out_host = head_wide_workspace_bytes_public(a, b, c) + 256; return ADN_OK;
+    case ADN_Q_METRICS_WORKSPACE_BYTES: *out_host = metrics::workspace_bytes(a, b, c); return ADN_OK;
     case ADN_Q_DENSE_FWD_PATH: *out_host = pick_fwd_path(a, b, c); return ADN_OK;
     case ADN_Q_DENSE_BWD_PATH: *out_host = pick_bwd_path(a, b, c); return ADN_OK;
     case ADN_Q_SM_COUNT: *out_host = sm_count(); return ADN_OK;

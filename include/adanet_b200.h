@@ -89,6 +89,7 @@ extern "C" {
 #define ADN_Q_TMA_MAP_CACHE_MISSES 14
 #define ADN_Q_HEAD_PATH 15                /* a=dim b=members -> 0: adn_head_group, 1: adn_head_group_wide */
 #define ADN_Q_HEAD_WIDE_WORKSPACE_BYTES 16 /* a=batch b=dim c=members (adn_head_group_wide) */
+#define ADN_Q_METRICS_WORKSPACE_BYTES 17  /* a=rows b=max dim c=ops (adn_metrics_group) */
 
 const char* adn_last_error(void);
 /* One-time, idempotent host-side initialisation (kernel attributes, driver entry
@@ -388,6 +389,48 @@ typedef struct adn_opt_op {
   const int64_t* cols_host;     /* nullable */
 } adn_opt_op;
 int adn_opt_step_group(const adn_opt_op* ops_host, int n, void* stream);
+
+/*
+ * Streaming evaluation metrics of the v2 BinaryClassHead and RegressionHead (AUC, precision, recall, means): the
+ * accumulator half of the tf.keras metrics that the reference's Evaluator streams every hold-out batch through
+ * (adanet/core/evaluator.py:97-140) and that Estimator.evaluate reports through the head's eval_metric_ops
+ * (adanet/core/eval_metrics.py:111-118).
+ * One op is one ensemble's fp32 logits [rows, dim] (the ens_out of its head) and its float labels [rows, dim]; the
+ * call ADDS the batch to the op's accumulators (the caller zeroes them when an evaluation starts):
+ *   sums[3] (fp64) += {sum of predictions, sum of labels, rows * dim}, where a prediction is the logit (MEANS) or
+ *     p = 1.f / (1.f + expf(-logit)) in fp32 (BINARY);
+ *   BINARY only, counts[ADN_METRICS_COUNTS] (int64) +=
+ *     [0, 201): histogram of the negative examples over buckets b = #{i : t_i < p}, thresholds t_0 = fp32(-1e-7),
+ *               t_i = fp32(i / 199) for i = 1..198, t_199 = fp32(1 + 1e-7) (Keras AUC(num_thresholds=200)); a NaN p
+ *               is in bucket 0 (predicted negative at every threshold);
+ *     [201, 402): the same histogram of the positive examples;
+ *     [402], [403]: negatives, positives with logit > 0 (class_ids = argmax([0, logit]) of the v2 binary head).
+ *   An example is positive when label > 0.5 (a NaN label is negative).  tp_i = sum_{b > i} positives[b] and so on
+ *   are suffix sums of the histograms, formed on the host with the metric formulas (adanet_b200/core/metrics.py).
+ * Counts are integer atomics; the sums go through per-CTA partials in `workspace` and one fixed-order finalize, and
+ * the CTA count is a function of (rows, max dim, n) alone, so results are bit-identical across runs and devices.
+ * One launch plus one finalize launch per 32 ops.  Every op is checked before anything is launched: n outside
+ * 1..ADN_METRICS_MAX_OPS, rows or dim < 1, a null pointer (counts may be NULL for MEANS), a bad kind or two ops
+ * sharing `sums` is ADN_ERR_INVALID, BINARY with dim != 1 ADN_ERR_UNSUPPORTED, a workspace smaller than
+ * adn_query(ADN_Q_METRICS_WORKSPACE_BYTES, rows, max dim, n) ADN_ERR_WORKSPACE; a rejected call changes no
+ * accumulator.
+ */
+#define ADN_METRICS_BINARY 0      /* dim == 1, sigmoid head: histograms, class-id counts and sums */
+#define ADN_METRICS_MEANS 1       /* regression head: sums only */
+#define ADN_METRICS_THRESHOLDS 200
+#define ADN_METRICS_COUNTS 404    /* 2 * (ADN_METRICS_THRESHOLDS + 1) + 2 */
+#define ADN_METRICS_MAX_OPS 1024
+typedef struct adn_metrics_op {
+  int32_t kind;             /* ADN_METRICS_* */
+  int32_t reserved;
+  const float* logits;      /* device [rows, dim] */
+  const float* labels_f;    /* device [rows, dim] */
+  int64_t dim;
+  int64_t* counts;          /* device [ADN_METRICS_COUNTS], accumulated; NULL for MEANS */
+  double* sums;             /* device [3], accumulated */
+} adn_metrics_op;
+int adn_metrics_group(const adn_metrics_op* ops_host, int n, int64_t rows, void* workspace, int64_t workspace_bytes,
+                      void* stream);
 
 /* out[0] = sum_i |x[i]| over n elements (tf.norm(ord=1), weighted.py:573), fixed order. */
 int adn_l1_norm(const float* x, int64_t n, float* out, void* stream);
