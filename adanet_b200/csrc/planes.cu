@@ -903,16 +903,23 @@ pl_gemm_ms_kernel(const __grid_constant__ MsGroup grp) {
 }
 
 // ---------------------------------------------------------------------------------
-// Wide dW kernel (pl_dw_kernel): the fp16 dW waves (EPI_PARTIAL) on 128 x 128 tiles.  pl_gemm_kernel's 128 x 64 tile
-// issues m64n64k16, whose 4 KiB of operands per 65,536 MACs take all of an SM's shared-memory bandwidth at the tensor
-// rate, and re-reads its A rows from L2 once per 64 output columns.  Here each consumer warpgroup owns 64 rows x 128
-// columns and issues m64n128k16 (6 KiB per 131,072 MACs), and A is read once per 128 columns.  A dW work item ends in
-// a plain fp32 store of its tile (the split-K partial, or dW itself with one split), so there is no epilogue
-// warpgroup: the consumers store their fragments straight from registers while the producer refills the ring, and the
-// register file goes to the three accumulators of 64 x 128 outputs (H, S and the RN-folded acc, 64 each).
-// Work items, split boundaries and the per-element arithmetic (bias-free start, f16_kblock_at, fold_chunk every 128 K,
-// out_mul) are pl_gemm_kernel's, so dW is bit-identical to it.  One thread of the producer warpgroup issues the TMA
-// loads: A_hi, A_lo', B_hi, B_lo' as MN-major [2][64 k][64 mn] boxes of 16 KiB each per k-block.
+// Wide kernels (pl_dw_kernel, pl_wide_kernel): fp16 groups on 128 x 128 tiles.  pl_gemm_kernel's 128 x 64 tile issues
+// m64n64k16, whose 4 KiB of operands per 65,536 MACs take all of an SM's shared-memory bandwidth at the tensor rate,
+// and re-reads its A rows from L2 once per 64 output columns.  Here each consumer warpgroup owns 64 rows x 128 columns
+// and issues m64n128k16 (6 KiB per 131,072 MACs), and A is read once per 128 columns.  There is no epilogue warpgroup:
+// the register file goes to the three accumulators of 64 x 128 outputs (H, S and the RN-folded acc, 64 each), and the
+// consumers run their own epilogue while the producer refills the ring with the next item's first k-blocks.
+//   pl_dw_kernel (EPI_PARTIAL, dW): the consumers store their fragments straight from registers as fp32 (the split-K
+//     partial, or dW itself with one split).
+//   pl_wide_kernel<EPI_BIAS_ACT | EPI_MASK> (forward / dX with planes out, single source): after the last fold H and S
+//     are dead, and each consumer warpgroup moves its 64 x 128 result through a private 16 KiB area one 64 x 64 unit
+//     at a time, as pl_thin_kernel does: fp32 staging tile, row-per-lane read, emit_slice_*_planes into the hi / lo'
+//     slabs that reuse the same area, one 64 x 64 TMA store per plane.
+// Work items, split boundaries and the per-element arithmetic (bias start, f16_kblock_at, fold_chunk every 128 K, the
+// epilogues of pl_gemm_kernel) are pl_gemm_kernel's; column sums go per 32-row slice, sign bits per 32 columns and the
+// dropout hash per element index, so every output byte is pl_gemm_kernel's.  One thread of the producer warpgroup
+// issues the TMA loads, 16 KiB per operand plane and k-block: A as K-major [128 rows][64 k] (fwd, dX) or MN-major
+// [2][64 k][64 mn] (dW) boxes, B as MN-major [2][64 k][64 n] (fwd, dW) or K-major [128 n][64 k] (dX) boxes.
 // ---------------------------------------------------------------------------------
 static constexpr int DW_BN = 128;
 static constexpr int DW_B_TILE = DW_BN * 128;                  // 16 KiB
@@ -923,14 +930,41 @@ static_assert(128 * PRODUCER_REGS + 128 * CONSUMERS * DW_CONSUMER_REGS <= 65536,
 static_assert(PRODUCER_REGS < 65536 / DW_THREADS && DW_CONSUMER_REGS > 65536 / DW_THREADS, "setmaxnreg.dec / .inc");
 static constexpr int DW_SMEM_BYTES = 1024 + STAGES * DW_STAGE_BYTES + BAR_BYTES;
 static_assert(DW_SMEM_BYTES <= 232448, "shared memory per block");
+// planes out: a consumer warpgroup's area, first its fp32 [64][64] staging tile, then its hi and lo' [64][64] fp16 slabs
+static constexpr int WIDE_AREA_BYTES = 64 * 64 * 4;
+static_assert(WIDE_AREA_BYTES == 2 * 64 * 128, "the staging tile and the two store slabs share the area");
+static constexpr int WIDE_SMEM_BYTES = DW_SMEM_BYTES + CONSUMERS * WIDE_AREA_BYTES;
+static_assert(WIDE_SMEM_BYTES <= 232448, "shared memory per block");
 
-__global__ void __launch_bounds__(DW_THREADS, 1)
-pl_dw_kernel(const __grid_constant__ Group grp) {
+// the lane's 32 values of row srow, columns scol.. of a 64 x 64 unit, into the hi and lo' [64 rows][128 B] slabs (16 B
+// chunk ^= row % 8, the SWIZZLE_128B layout of the 64 x 64 store boxes); the emit_slice_*_planes store path of
+// pl_thin_kernel and pl_wide_kernel
+struct SlabStore64 {
+  uint32_t slab_hi, slab_lo;
+  int srow, scol;
+  __device__ __forceinline__ void operator()(const float* v) const {
+    uint32_t w[16], lw[16];
+    split_f16x32(v, w, lw);
+    const uint32_t roff = (uint32_t)srow * 128u, sw = (uint32_t)srow & 7u, c0 = (uint32_t)scol >> 3;
+#pragma unroll
+    for (uint32_t q = 0; q < 4; ++q) {
+      sts_v4(slab_hi + roff + (((c0 + q) ^ sw) << 4), w[4 * q], w[4 * q + 1], w[4 * q + 2], w[4 * q + 3]);
+      sts_v4(slab_lo + roff + (((c0 + q) ^ sw) << 4), lw[4 * q], lw[4 * q + 1], lw[4 * q + 2], lw[4 * q + 3]);
+    }
+  }
+};
+
+template <int EPI>
+__device__ __forceinline__ void pl_wide_body(const Group& grp) {
   constexpr int BK = Fmt<FMT_F16>::BK;
   constexpr int CHUNK = Fmt<FMT_F16>::CHUNK;
+  constexpr bool PLANES = EPI != EPI_PARTIAL;
+  constexpr int A_MN = EPI == EPI_PARTIAL, B_MN = EPI != EPI_MASK;   // operand majorness of fwd / dX / dW
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * DW_STAGE_BYTES);
+  // the ring, the consumer warpgroups' areas (planes out; 1024 B aligned for the SWIZZLE_128B store boxes), the barriers
+  uint8_t* areas = smem + STAGES * DW_STAGE_BYTES;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(areas + (PLANES ? CONSUMERS * WIDE_AREA_BYTES : 0));
   uint64_t* full_bar = bars;                       // [STAGES]  TMA -> consumers
   uint64_t* empty_bar = bars + STAGES;             // [STAGES]  consumers -> TMA, count CONSUMER_WARPS
 
@@ -970,11 +1004,14 @@ pl_dw_kernel(const __grid_constant__ Group grp) {
           mbar_expect_tx(fb, DW_STAGE_BYTES);
           const uint32_t base = smem0 + s * DW_STAGE_BYTES;
           const int kc = it.kb0 + kb;
-          // MN-major boxes {BK, BK k-rows, 2 blocks of 64 columns} at (0, kc * BK, mn0 / BK)
-          tma_load_3d(&pr.a_hi, fb, base, 0, kc * BK, it.m0 / BK);
-          tma_load_3d(&pr.a_lo, fb, base + A_TILE, 0, kc * BK, it.m0 / BK);
-          tma_load_3d(&pr.b_hi, fb, base + 2 * A_TILE, 0, kc * BK, it.n0 / BK);
-          tma_load_3d(&pr.b_lo, fb, base + 2 * A_TILE + DW_B_TILE, 0, kc * BK, it.n0 / BK);
+          // K-major box {BK, 128 rows, 1 kb} at (0, row0, kc); MN-major box {BK, BK k-rows, 2 blocks of 64} at
+          // (0, kc * BK, mn0 / BK)
+          const int a1 = A_MN ? kc * BK : it.m0, a2 = A_MN ? it.m0 / BK : kc;
+          const int b1 = B_MN ? kc * BK : it.n0, b2 = B_MN ? it.n0 / BK : kc;
+          tma_load_3d(&pr.a_hi, fb, base, 0, a1, a2);
+          tma_load_3d(&pr.a_lo, fb, base + A_TILE, 0, a1, a2);
+          tma_load_3d(&pr.b_hi, fb, base + 2 * A_TILE, 0, b1, b2);
+          tma_load_3d(&pr.b_lo, fb, base + 2 * A_TILE + DW_B_TILE, 0, b1, b2);
           if (++s == STAGES) { s = 0; ph ^= 1; }
         }
       }
@@ -990,16 +1027,45 @@ pl_dw_kernel(const __grid_constant__ Group grp) {
   const uint32_t smem0 = smem_u32(smem);
   uint32_t s = 0, ph = 0;
   int cur = 0, next0 = first_next0(grp);
-  float H[64], S[64];                              // MMA accumulators of one 128-K chunk
+  float H_[64], S_[64];                            // MMA accumulators of one 128-K chunk
 #pragma unroll
-  for (int j = 0; j < 64; ++j) H[j] = S[j] = 0.f;
+  for (int j = 0; j < 64; ++j) H_[j] = S_[j] = 0.f;
   for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
     cur = find_problem(grp, cur, item, next0);
     const GemmParams& g = grp.p[cur].g;
     const Item it = decode_item<DW_BN>(g, item - grp.p[cur].item0);
+    float(&H)[64] = H_;
+    float(&S)[64] = S_;
+    if constexpr (PLANES) {
+      // ends the live range of the previous item's H and S before its epilogue, which needs their registers (the
+      // first MMA of every chunk overwrites them)
+#pragma unroll
+      for (int j = 0; j < 64; ++j) H[j] = S[j] = 0.f;
+    }
+    // planes out: this warp's 32 x 32 slice of each 64 x 64 unit (row per lane), and the global words the epilogue
+    // needs, loaded before the MMAs: the ReLU-mask words of the lane's row (dX; all ones without a mask, 0 past M or
+    // the last 32-column block) and the dropout step
+    [[maybe_unused]] const int srow = 32 * (wq >> 1) + lane, scol = 32 * (wq & 1);
+    [[maybe_unused]] uint32_t mw[2] = {0xffffffffu, 0xffffffffu}, drop_step = 0u;
+    if constexpr (EPI == EPI_MASK) {
+      if (g.mask_bits) {
+        const int my_row = it.m0 + 64 * wgi + srow, kbo = (it.n0 + scol) >> 5;
+#pragma unroll
+        for (int u = 0; u < 2; ++u)
+          mw[u] = (my_row < g.M && kbo + 2 * u < g.out_nb32) ? __ldg(g.mask_bits + (size_t)(kbo + 2 * u) * g.M + my_row) : 0u;
+      }
+    }
+    if constexpr (EPI == EPI_BIAS_ACT) drop_step = g.drop_thresh != 0u ? (uint32_t)(*g.drop_step) : 0u;
     float acc[64];
 #pragma unroll
-    for (int j = 0; j < 64; ++j) acc[j] = 0.f;
+    for (int j = 0; j < 64; ++j) {
+      if constexpr (EPI == EPI_BIAS_ACT) {       // the bias starts the accumulation
+        const int col = it.n0 + 8 * (j >> 2) + 2 * tq + (j & 1);
+        acc[j] = (g.bias && col < g.N) ? __ldg(g.bias + col) : 0.f;
+      } else {
+        acc[j] = 0.f;
+      }
+    }
     for (int kb = 0; kb < it.nkb; ++kb) {
       const bool first = (kb % CHUNK) == 0;
       const bool last = (kb % CHUNK) == CHUNK - 1 || kb == it.nkb - 1;
@@ -1008,7 +1074,7 @@ pl_dw_kernel(const __grid_constant__ Group grp) {
       wg::fence_regs(S);
       wg::fence();
       const uint32_t st = smem0 + s * DW_STAGE_BYTES;
-      f16_kblock_at<1, 1, DW_BN>(st + (uint32_t)wgi * 8192u, st + 2 * A_TILE, H, S, first);
+      f16_kblock_at<A_MN, B_MN, DW_BN>(st + (uint32_t)wgi * 8192u, st + 2 * A_TILE, H, S, first);
       wg::commit();
       wg::wait<0>();
       wg::fence_regs(H);
@@ -1018,31 +1084,90 @@ pl_dw_kernel(const __grid_constant__ Group grp) {
       if (++s == STAGES) { s = 0; ph ^= 1; }
       if (last) fold_chunk<FMT_F16>(acc, H, S);
     }
-    // ---- the tile leaves from the fragment layout: a quad holds 8 consecutive columns (one 32 B sector) of a row ----
-    float* dense = reinterpret_cast<float*>(g.out) + (size_t)it.split * g.M * g.N;
-    const bool vec = (g.ldc & 1) == 0 && (reinterpret_cast<uintptr_t>(dense) & 7) == 0;
-    if (g.out_mul != 1.0f) {
+    if constexpr (EPI == EPI_PARTIAL) {
+      // ---- the tile leaves from the fragment layout: a quad holds 8 consecutive columns (one 32 B sector) of a row ----
+      float* dense = reinterpret_cast<float*>(g.out) + (size_t)it.split * g.M * g.N;
+      const bool vec = (g.ldc & 1) == 0 && (reinterpret_cast<uintptr_t>(dense) & 7) == 0;
+      if (g.out_mul != 1.0f) {
 #pragma unroll
-      for (int j = 0; j < 64; ++j) acc[j] *= g.out_mul;
-    }
+        for (int j = 0; j < 64; ++j) acc[j] *= g.out_mul;
+      }
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int row = it.m0 + 64 * wgi + 16 * wq + gid + 8 * h;
-      if (row >= g.M) continue;
-      float* rp = dense + (size_t)row * g.ldc;
+      for (int h = 0; h < 2; ++h) {
+        const int row = it.m0 + 64 * wgi + 16 * wq + gid + 8 * h;
+        if (row >= g.M) continue;
+        float* rp = dense + (size_t)row * g.ldc;
 #pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const int col = it.n0 + 8 * j + 2 * tq;
-        const float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-        if (vec && col + 1 < g.N) {
-          *reinterpret_cast<float2*>(rp + col) = make_float2(v0, v1);
-        } else {
-          if (col < g.N) rp[col] = v0;
-          if (col + 1 < g.N) rp[col + 1] = v1;
+        for (int j = 0; j < 16; ++j) {
+          const int col = it.n0 + 8 * j + 2 * tq;
+          const float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+          if (vec && col + 1 < g.N) {
+            *reinterpret_cast<float2*>(rp + col) = make_float2(v0, v1);
+          } else {
+            if (col < g.N) rp[col] = v0;
+            if (col + 1 < g.N) rp[col + 1] = v1;
+          }
         }
       }
+    } else {
+      // ---- two 64 x 64 units: fragment layout -> staging tile -> row per lane -> slabs -> TMA stores ----
+      // The thread's coordinates are read again here: the shared addresses derived from them are loop-invariant, and
+      // hoisted out of the item loop they stayed live through the mainloop and were spilled.
+      uint32_t tid;
+      asm volatile("mov.u32 %0, %%tid.x;" : "=r"(tid));
+      const int lane = tid & 31, wq = (tid >> 5) & 3, gid = lane >> 2, tq = lane & 3;
+      const int srow = 32 * (wq >> 1) + lane, scol = 32 * (wq & 1);
+      const Problem& pr = grp.p[cur];
+      const uint32_t area = smem_u32(areas) + (uint32_t)wgi * WIDE_AREA_BYTES;
+      const SlabStore64 store16{area, area + WIDE_AREA_BYTES / 2, srow, scol};
+      const int mrow0 = it.m0 + 64 * wgi + 32 * (wq >> 1);
+#pragma unroll
+      for (int u = 0; u < 2; ++u) {
+        const int n0 = it.n0 + 64 * u;
+        if (n0 >= 32 * g.out_nb32) continue;       // warpgroup-uniform: the unit lies past the padded output
+        // past this barrier the warpgroup's previous slices have been read and its previous stores have read the
+        // area (the issuing thread waited for them)
+        if (wq == 0 && lane == 0) bulk_wait_read0();
+        asm volatile("bar.sync %0, 128;" ::"r"(1 + wgi) : "memory");
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+          const int row = 16 * wq + gid, col = 8 * jj + 2 * tq, j = 8 * u + jj;
+          sts_v2(area + 4u * acc_off(row, col), acc[4 * j], acc[4 * j + 1]);
+          sts_v2(area + 4u * acc_off(row + 8, col), acc[4 * j + 2], acc[4 * j + 3]);
+        }
+        asm volatile("bar.sync %0, 128;" ::"r"(1 + wgi) : "memory");
+        float a[32];
+#pragma unroll
+        for (int q = 0; q < 8; ++q) lds_v4(area + 4u * acc_off(srow, scol + 4 * q), a[4 * q], a[4 * q + 1], a[4 * q + 2], a[4 * q + 3]);
+        // every warp has read the staging tile before the slabs overwrite it
+        asm volatile("bar.sync %0, 128;" ::"r"(1 + wgi) : "memory");
+        if constexpr (EPI == EPI_BIAS_ACT)
+          emit_slice_fwd_planes<FMT_F16>(g, a, drop_step, lane, mrow0, n0 + scol, nullptr, nullptr, 0u, 0u, &store16);
+        else
+          emit_slice_mask_planes<FMT_F16>(g, a, mw[u], lane, mrow0, n0 + scol, nullptr, nullptr, 0u, 0u, &store16);
+        fence_async_smem();
+        asm volatile("bar.sync %0, 128;" ::"r"(1 + wgi) : "memory");
+        if (wq == 0 && lane == 0) {
+          tma_store_3d(&pr.o_hi, store16.slab_hi, 0, it.m0 + 64 * wgi, n0 / BK);
+          tma_store_3d(&pr.o_lo, store16.slab_lo, 0, it.m0 + 64 * wgi, n0 / BK);
+          bulk_commit();
+        }
+      }
+      // stores complete before the CTA (and its shared memory) goes away.  (Inside the loop: with this wait after it,
+      // ptxas kept the consumers to 192 registers and spilled the accumulators.)
+      if (item + (int)gridDim.x >= n_items && wq == 0 && lane == 0) bulk_wait0();
     }
   }
+}
+
+__global__ void __launch_bounds__(DW_THREADS, 1)
+pl_dw_kernel(const __grid_constant__ Group grp) {
+  pl_wide_body<EPI_PARTIAL>(grp);
+}
+template <int EPI>
+__global__ void __launch_bounds__(DW_THREADS, 1)
+pl_wide_kernel(const __grid_constant__ Group grp) {
+  pl_wide_body<EPI>(grp);
 }
 
 // ---------------------------------------------------------------------------------
@@ -1222,19 +1347,10 @@ pl_thin_kernel(const __grid_constant__ Group grp) {
       float a[32];
 #pragma unroll
       for (int q = 0; q < 8; ++q) lds_v4(stage + 4u * acc_off(srow, scol + 4 * q), a[4 * q], a[4 * q + 1], a[4 * q + 2], a[4 * q + 3]);
-      // the lane's row of each plane goes into the warpgroup's [64 rows][128 B] slabs (16 B chunk ^= row % 8, the
-      // SWIZZLE_128B layout); one thread then stores the 64 x 64 unit of each plane with a single TMA store, 128 B
-      // per row, instead of four 32 x 32 boxes of 64 B rows per plane
-      const auto store16 = [&](const float* v) {
-        uint32_t w[16], lw[16];
-        split_f16x32(v, w, lw);
-        const uint32_t roff = (uint32_t)srow * 128u, sw = (uint32_t)srow & 7u, c0 = (uint32_t)scol >> 3;
-#pragma unroll
-        for (uint32_t q = 0; q < 4; ++q) {
-          sts_v4(slab_hi + roff + (((c0 + q) ^ sw) << 4), w[4 * q], w[4 * q + 1], w[4 * q + 2], w[4 * q + 3]);
-          sts_v4(slab_lo + roff + (((c0 + q) ^ sw) << 4), lw[4 * q], lw[4 * q + 1], lw[4 * q + 2], lw[4 * q + 3]);
-        }
-      };
+      // the lane's row of each plane goes into the warpgroup's [64 rows][128 B] slabs; one thread then stores the
+      // 64 x 64 unit of each plane with a single TMA store, 128 B per row, instead of four 32 x 32 boxes of 64 B rows
+      // per plane
+      const SlabStore64 store16{slab_hi, slab_lo, srow, scol};
       const int mrow0 = mb * BM + 64 * half + 32 * (wq >> 1), cbase = n0 + scol;
       if (EPI == EPI_BIAS_ACT) {
         const uint32_t drop_step = g.drop_thresh != 0u ? (uint32_t)(*g.drop_step) : 0u;
@@ -1396,6 +1512,8 @@ int init() {
     ok = ok && cudaFuncSetAttribute(pl_thin_kernel<EPI_BIAS_ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, THIN_SMEM_BYTES) == cudaSuccess;
     ok = ok && cudaFuncSetAttribute(pl_thin_kernel<EPI_MASK>, cudaFuncAttributeMaxDynamicSharedMemorySize, THIN_SMEM_BYTES) == cudaSuccess;
     ok = ok && cudaFuncSetAttribute(pl_dw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DW_SMEM_BYTES) == cudaSuccess;
+    ok = ok && cudaFuncSetAttribute(pl_wide_kernel<EPI_BIAS_ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, WIDE_SMEM_BYTES) == cudaSuccess;
+    ok = ok && cudaFuncSetAttribute(pl_wide_kernel<EPI_MASK>, cudaFuncAttributeMaxDynamicSharedMemorySize, WIDE_SMEM_BYTES) == cudaSuccess;
     if (!ok) {
       (void)cudaGetLastError();
       rc = fail(ADN_ERR_CUDA, "pl::init: cudaFuncSetAttribute(smem=%d) failed", SMEM_BYTES);
@@ -1485,7 +1603,7 @@ static int make_map(int fmt, CUtensorMap* map, const void* plane, int64_t rows, 
 }
 
 // output planes (fp16) as TMA store targets: [box columns][box rows] boxes; box = 32 (pl_gemm_kernel's 32 x 32 slices,
-// 64 B rows, SWIZZLE_64B in shared memory) or 64 (pl_thin_kernel's 64 x 64 units, 128 B rows, SWIZZLE_128B)
+// 64 B rows, SWIZZLE_64B in shared memory) or 64 (pl_thin_kernel's and pl_wide_kernel's 64 x 64 units, 128 B rows, SWIZZLE_128B)
 static int make_store_map(CUtensorMap* map, const void* plane, int64_t rows, int64_t nkb, int box_rc = 32) {
   if (!g_encode) return fail(ADN_ERR_CUDA, "pl: adn_init() was not called");
   const MapKey key{plane, rows, nkb, 2, FMT_F16, box_rc};      // mn = 2: a store box
@@ -1564,6 +1682,42 @@ static bool dw_group(int fmt, const Group& grp) {
   const int64_t sms = sm_count();
   return 8 * wide <= 9 * narrow && 2 * ceil_div(items_w, sms) <= ceil_div(items_n, sms) + 1;
 }
+// MMA work (k-blocks x tile columns) of the busiest CTA when the group's work items are dealt round-robin, tiles of
+// `bn` columns.  Problem i's items are a contiguous run, so CTA c gets full or full + 1 of them: O(problems x SMs).
+static int64_t busiest_cta_work(const Group& grp, int bn) {
+  int64_t items = 0;
+  for (int i = 0; i < grp.n; ++i) items += ceil_div(grp.p[i].g.M, BM) * ceil_div(grp.p[i].g.N, bn) * grp.p[i].g.splits;
+  const int64_t ctas = std::min<int64_t>(items, sm_count());
+  if (ctas <= 0) return 0;
+  std::vector<int64_t> work((size_t)ctas, 0);
+  int64_t j0 = 0;
+  for (int i = 0; i < grp.n; ++i) {
+    const GemmParams& g = grp.p[i].g;
+    const int64_t cnt = ceil_div(g.M, BM) * ceil_div(g.N, bn) * g.splits, w = (int64_t)g.kb_per_split * bn;
+    const int64_t full = cnt / ctas, rem = cnt % ctas, first = j0 % ctas;
+    for (int64_t c = 0; c < ctas; ++c) work[(size_t)c] += w * (full + ((c - first + ctas) % ctas < rem ? 1 : 0));
+    j0 += cnt;
+  }
+  return *std::max_element(work.begin(), work.end());
+}
+// A single-source forward or dX group runs on pl_wide_kernel when the format is fp16, every problem has planes out,
+// the group is not a thin-K group (pl_thin_kernel keeps those), padding every problem's N to 128 columns adds at most
+// 1/8 to the group's MMA work, and so does the wide tile to the busiest CTA's.  The second bound counts work, not
+// rounds as dw_group does: the layer waves mix problems of 1 to 16 k-blocks per item.  (The hidden-layer waves of the
+// benchmarked step deal 6,912 wide items in 53 rounds against 13,312 narrow ones in 101, which dw_group's rule
+// refuses, but the busiest CTA gets 1,052 k-blocks of 64 columns against 1,038.)  Dense fp32 outputs (the logits
+// forward, the conv stem's dX) and TF32 planes stay on pl_gemm_kernel.
+static bool wide_group(int fmt, const Group& grp) {
+  if (fmt != FMT_F16 || thin_group(fmt, grp)) return false;
+  int64_t narrow = 0, wide = 0;
+  for (int i = 0; i < grp.n; ++i) {
+    const GemmParams& g = grp.p[i].g;
+    if (!g.out_planes) return false;
+    narrow += ceil_div(g.M, BM) * g.total_kb * ceil_div(g.N, BN) * BN;
+    wide += ceil_div(g.M, BM) * g.total_kb * ceil_div(g.N, DW_BN) * DW_BN;
+  }
+  return 8 * wide <= 9 * narrow && 8 * busiest_cta_work(grp, DW_BN) <= 9 * busiest_cta_work(grp, BN);
+}
 template <int FMT, int EPI>
 static void launch_kernel(const Group& grp, int grid, cudaStream_t st) {
   pl_gemm_kernel<FMT, EPI><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(grp);
@@ -1582,12 +1736,13 @@ static int build_groups(int fmt, const GemmDesc* d, int n, std::vector<G>& out, 
       out.emplace_back();
       G& grp = out.back();
       memset(&grp, 0, sizeof(grp));
-      // the tile width: 128 columns when the dW group goes to pl_dw_kernel (dw_group reads only the shapes set here)
+      // the tile width: 128 columns when the group goes to pl_dw_kernel or pl_wide_kernel (dw_group and wide_group
+      // read only the parameters set here)
       int bn = BN;
-      if constexpr (!MS && EPI == EPI_PARTIAL) {
+      if constexpr (!MS) {
         for (int i = 0; i < m; ++i) grp.p[i].g = d[i0 + i].g;
         grp.n = m;
-        if (dw_group(fmt, grp)) bn = DW_BN;
+        if (EPI == EPI_PARTIAL ? dw_group(fmt, grp) : wide_group(fmt, grp)) bn = DW_BN;
       }
       int items = 0;
       for (int i = 0; i < m; ++i) {
@@ -1613,10 +1768,12 @@ static int build_groups(int fmt, const GemmDesc* d, int n, std::vector<G>& out, 
           if (kb != src.g.total_kb) return fail(ADN_ERR_INVALID, "%s: k-blocks of the pieces do not add up", what);
         }
         pr.g = src.g;
-        // fp16 plane tiles leave the epilogue by TMA stores (the API checked yp / dxp against planes_aligned)
+        // fp16 plane tiles leave the epilogue by TMA stores (the API checked yp / dxp against planes_aligned):
+        // pl_gemm_kernel's 32 x 32 slices, or pl_wide_kernel's 64 x 64 units
         if (fmt == FMT_F16 && src.g.out_planes) {
-          if ((rc = make_store_map(&pr.o_hi, src.g.out, src.g.M, src.g.out_nb32 / 2))) return rc;
-          if ((rc = make_store_map(&pr.o_lo, src.g.out_lo, src.g.M, src.g.out_nb32 / 2))) return rc;
+          const int box = bn == DW_BN ? 64 : 32;
+          if ((rc = make_store_map(&pr.o_hi, src.g.out, src.g.M, src.g.out_nb32 / 2, box))) return rc;
+          if ((rc = make_store_map(&pr.o_lo, src.g.out_lo, src.g.M, src.g.out_nb32 / 2, box))) return rc;
         }
         pr.g.a_mn = src.a.mn_major;
         pr.g.b_mn = src.b.mn_major;
@@ -1662,6 +1819,8 @@ static int launch_groups(int fmt, const std::vector<G>& groups, cudaStream_t st,
       if constexpr (EPI != EPI_PARTIAL) pl_thin_kernel<EPI><<<grid, THIN_THREADS, THIN_SMEM_BYTES, st>>>(grp);
     } else if (EPI == EPI_PARTIAL && dw_group(fmt, grp)) {
       pl_dw_kernel<<<grid, DW_THREADS, DW_SMEM_BYTES, st>>>(grp);
+    } else if (EPI != EPI_PARTIAL && wide_group(fmt, grp)) {
+      if constexpr (EPI != EPI_PARTIAL) pl_wide_kernel<EPI><<<grid, DW_THREADS, WIDE_SMEM_BYTES, st>>>(grp);
     } else {
       if (fmt == FMT_F16) launch_kernel<FMT_F16, EPI>(grp, grid, st);
       else launch_kernel<FMT_TF32, EPI>(grp, grid, st);

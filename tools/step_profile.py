@@ -71,7 +71,7 @@ def classify(name):
   m = re.search(r"pl_gemm_kernel<(\d+), (\d+)>", name)
   if m:
     return "gemm", int(m.group(2))
-  m = re.search(r"pl_thin_kernel<(\d+)>", name)
+  m = re.search(r"pl_(?:thin|wide)_kernel<(\d+)>", name)
   if m:
     return "gemm", int(m.group(1))
   if "pl_dw_kernel" in name:
