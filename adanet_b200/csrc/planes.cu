@@ -296,12 +296,11 @@ __device__ __forceinline__ void store_slice_tma(const CUtensorMap* o_hi, const C
 
 // Forward epilogue with planes out, WITHOUT a register transpose: lane = row keeps its 32 accumulators (bias already
 // added by the caller), applies ReLU / dropout, forms the sign-bit word, splits pairs of values with packed conversions
-// and hands its 32 columns of each plane to the slab + TMA store path (fp16) or writes them with direct 16 B stores
-// (TF32: 128 B per plane).  A caller with its own fp16 store path passes it as `store16` (the maps and slabs unused).
-template <int FMT, class Store16 = void>
+// and hands its 32 columns of both planes to `store` (the caller's plane store path: store_slice_tma or SlabStore64 for
+// fp16, store_row32_tf32 for TF32).
+template <class Store>
 __device__ __forceinline__ void emit_slice_fwd_planes(const GemmParams& g, float* a, uint32_t drop_step, int lane, int mrow0,
-                                                      int cbase, const CUtensorMap* o_hi, const CUtensorMap* o_lo,
-                                                      uint32_t slab_hi, uint32_t slab_lo, const Store16* store16 = nullptr) {
+                                                      int cbase, const Store& store) {
   const int my_row = mrow0 + lane;
   const int kbo = cbase >> 5;
   if (kbo >= g.out_nb32) return;                         // warp-uniform
@@ -327,9 +326,7 @@ __device__ __forceinline__ void emit_slice_fwd_planes(const GemmParams& g, float
     for (int j = 0; j < 32; ++j)
       if (!((cmask >> j) & 1u)) a[j] = 0.f;
   }
-  if constexpr (!std::is_void<Store16>::value) (*store16)(a);
-  else if (FMT == FMT_F16) store_slice_tma(o_hi, o_lo, slab_hi, slab_lo, a, lane, mrow0, cbase);
-  else if (my_row < g.M) store_row32_tf32(g, a, my_row, cbase);
+  store(a);
   uint32_t bits = 0u;
 #pragma unroll
   for (int j = 0; j < 32; ++j) bits |= (a[j] > 0.f) ? (1u << j) : 0u;
@@ -350,15 +347,14 @@ __device__ __forceinline__ void colsum_round(float* a, int lane) {
   }
 }
 
-// dX epilogue with planes out, without a register transpose: sign-bit ReLU mask, plane stores as in the forward
-// epilogue (slab + TMA for fp16 or the caller's `store16`, direct stores from the row-owning lane for TF32), and the per-32-row column sums
+// dX epilogue with planes out, without a register transpose: sign-bit ReLU mask, plane stores through `store` as in
+// the forward epilogue, and the per-32-row column sums
 // (the bias gradient of the layer below) by a butterfly over the warp: at distance w a lane keeps the half of its
 // columns selected by bit w of its lane id and receives the partner's partial sums for them, so after five rounds
 // lane l holds the sum of column l over the 32 rows (31 shuffles and adds per lane, fixed order).
-template <int FMT, class Store16 = void>
+template <class Store>
 __device__ __forceinline__ void emit_slice_mask_planes(const GemmParams& g, float* a, uint32_t mwq, int lane, int mrow0, int cbase,
-                                                       const CUtensorMap* o_hi, const CUtensorMap* o_lo, uint32_t slab_hi,
-                                                       uint32_t slab_lo, const Store16* store16 = nullptr) {
+                                                       const Store& store) {
   const int my_row = mrow0 + lane;
   const int kbo = cbase >> 5;
   if (kbo >= g.out_nb32) return;                         // warp-uniform
@@ -373,9 +369,7 @@ __device__ __forceinline__ void emit_slice_mask_planes(const GemmParams& g, floa
     for (int j = 0; j < 32; ++j)
       if (!((keep >> j) & 1u)) a[j] = 0.f;
   }
-  if constexpr (!std::is_void<Store16>::value) (*store16)(a);
-  else if (FMT == FMT_F16) store_slice_tma(o_hi, o_lo, slab_hi, slab_lo, a, lane, mrow0, cbase);
-  else if (my_row < g.M) store_row32_tf32(g, a, my_row, cbase);
+  store(a);
   if (g.colsum_part) {
     colsum_round<16>(a, lane);
     colsum_round<8>(a, lane);
@@ -387,6 +381,24 @@ __device__ __forceinline__ void emit_slice_mask_planes(const GemmParams& g, floa
   }
 }
 
+// pl_gemm_kernel's plane stores for the emitters above: a warp's fp16 slice through its hi and lo' slabs, a lane's TF32
+// row directly
+struct TmaSliceStore {
+  const CUtensorMap *o_hi, *o_lo;
+  uint32_t slab_hi, slab_lo;
+  int lane, mrow0, cbase;
+  __device__ __forceinline__ void operator()(const float* a) const {
+    store_slice_tma(o_hi, o_lo, slab_hi, slab_lo, a, lane, mrow0, cbase);
+  }
+};
+struct Tf32RowStore {
+  const GemmParams* g;
+  int my_row, cbase;
+  __device__ __forceinline__ void operator()(const float* a) const {
+    if (my_row < g->M) store_row32_tf32(*g, a, my_row, cbase);
+  }
+};
+
 // One 32-row x 32-column slice of a tile: lane = row holds its 32 accumulators a[0..31] (columns cbase..cbase+31,
 // the bias already in them).  Plane outputs go to the two functions above.  Everything else is a dense fp32 output
 // (the logits y, the conv stem's dense dX, the dW split-K partials): ReLU, or the scale and the sign-bit ReLU mask,
@@ -397,14 +409,14 @@ template <int FMT, int EPI>
 __device__ __forceinline__ void emit_slice(const GemmParams& g, const bool out_planes, float* a, uint32_t mwq, float* stage,
                                            int lane, int mrow0, int cbase, int rows_ok, float* dense, bool dense_vec,
                                            const CUtensorMap* o_hi, const CUtensorMap* o_lo, uint32_t drop_step) {
-  // `stage` is the warp's hi slab; its lo' slab follows it
-  if (EPI == EPI_BIAS_ACT && out_planes) {
-    emit_slice_fwd_planes<FMT>(g, a, drop_step, lane, mrow0, cbase, o_hi, o_lo, smem_u32(stage),
-                               smem_u32(stage + EPI_STAGE_FLOATS));
-    return;
-  }
-  if (EPI == EPI_MASK && out_planes) {
-    emit_slice_mask_planes<FMT>(g, a, mwq, lane, mrow0, cbase, o_hi, o_lo, smem_u32(stage), smem_u32(stage + EPI_STAGE_FLOATS));
+  // planes out: fp16 slices leave through the warp's hi slab `stage` and the lo' slab after it, TF32 rows directly
+  if (out_planes && EPI != EPI_PARTIAL) {
+    using Store = std::conditional_t<FMT == FMT_F16, TmaSliceStore, Tf32RowStore>;
+    Store store;
+    if constexpr (FMT == FMT_F16) store = {o_hi, o_lo, smem_u32(stage), smem_u32(stage + EPI_STAGE_FLOATS), lane, mrow0, cbase};
+    else store = {&g, mrow0 + lane, cbase};
+    if (EPI == EPI_BIAS_ACT) emit_slice_fwd_planes(g, a, drop_step, lane, mrow0, cbase, store);
+    else emit_slice_mask_planes(g, a, mwq, lane, mrow0, cbase, store);
     return;
   }
   constexpr int SW = 16;                   // staged columns per pass (2 KB per warp, two passes)
@@ -505,7 +517,7 @@ static constexpr int MAX_GROUP = 8;
 
 struct alignas(64) Problem {
   CUtensorMap a_hi, a_lo, b_hi, b_lo;
-  CUtensorMap o_hi, o_lo;   // fp16 output planes as [32 rows][32 columns] store boxes
+  CUtensorMap o_hi, o_lo;   // fp16 output planes as the kernel's store boxes (32 x 32 or 64 x 64)
   GemmParams g;
   int item0;             // first work item of this problem
   int pad_[3];
@@ -1142,9 +1154,9 @@ __device__ __forceinline__ void pl_wide_body(const Group& grp) {
         // every warp has read the staging tile before the slabs overwrite it
         asm volatile("bar.sync %0, 128;" ::"r"(1 + wgi) : "memory");
         if constexpr (EPI == EPI_BIAS_ACT)
-          emit_slice_fwd_planes<FMT_F16>(g, a, drop_step, lane, mrow0, n0 + scol, nullptr, nullptr, 0u, 0u, &store16);
+          emit_slice_fwd_planes(g, a, drop_step, lane, mrow0, n0 + scol, store16);
         else
-          emit_slice_mask_planes<FMT_F16>(g, a, mw[u], lane, mrow0, n0 + scol, nullptr, nullptr, 0u, 0u, &store16);
+          emit_slice_mask_planes(g, a, mw[u], lane, mrow0, n0 + scol, store16);
         fence_async_smem();
         asm volatile("bar.sync %0, 128;" ::"r"(1 + wgi) : "memory");
         if (wq == 0 && lane == 0) {
@@ -1354,10 +1366,10 @@ pl_thin_kernel(const __grid_constant__ Group grp) {
       const int mrow0 = mb * BM + 64 * half + 32 * (wq >> 1), cbase = n0 + scol;
       if (EPI == EPI_BIAS_ACT) {
         const uint32_t drop_step = g.drop_thresh != 0u ? (uint32_t)(*g.drop_step) : 0u;
-        emit_slice_fwd_planes<FMT_F16>(g, a, drop_step, lane, mrow0, cbase, nullptr, nullptr, 0u, 0u, &store16);
+        emit_slice_fwd_planes(g, a, drop_step, lane, mrow0, cbase, store16);
       }
       else
-        emit_slice_mask_planes<FMT_F16>(g, a, mw, lane, mrow0, cbase, nullptr, nullptr, 0u, 0u, &store16);
+        emit_slice_mask_planes(g, a, mw, lane, mrow0, cbase, store16);
       fence_async_smem();
       asm volatile("bar.sync %0, 128;" ::"r"(1 + wgi) : "memory");
       if (wq == 0 && lane == 0) {
@@ -1457,6 +1469,42 @@ merge_kernel(const void* __restrict__ hi_, const void* __restrict__ lo_, float* 
 // ---------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------
+// The kernel that runs a group, chosen once per group by choose_kernel when the group is built.
+enum class Kernel { GEMM, GEMM_MS, THIN, DW, WIDE };
+
+// What a kernel makes of a group: the tile width its work items count, how they are numbered, the TMA store boxes of
+// fp16 planes out, its launch shape, and its entry points by [format][epilogue kind] (null: no such instantiation).
+struct KernelSpec {
+  int tbn;               // tile columns: tiles_n counts tiles of this width
+  bool row_runs;         // items are 128-row blocks x runs of THIN_RUN N tiles, not tiles x splits
+  int store_box;         // fp16 planes out leave in store_box x store_box boxes (0: the kernel writes no planes)
+  int threads, smem;
+  const void* fn[2][3];
+};
+#define ADN_K(...) reinterpret_cast<const void*>(__VA_ARGS__)
+static const KernelSpec kSpecs[] = {
+    // Kernel::GEMM: pl_gemm_kernel's 32 x 32 slices
+    {BN, false, 32, NUM_THREADS, SMEM_BYTES,
+     {{ADN_K(pl_gemm_kernel<FMT_TF32, EPI_BIAS_ACT>), ADN_K(pl_gemm_kernel<FMT_TF32, EPI_MASK>),
+       ADN_K(pl_gemm_kernel<FMT_TF32, EPI_PARTIAL>)},
+      {ADN_K(pl_gemm_kernel<FMT_F16, EPI_BIAS_ACT>), ADN_K(pl_gemm_kernel<FMT_F16, EPI_MASK>),
+       ADN_K(pl_gemm_kernel<FMT_F16, EPI_PARTIAL>)}}},
+    // Kernel::GEMM_MS
+    {BN, false, 32, NUM_THREADS, SMEM_BYTES,
+     {{ADN_K(pl_gemm_ms_kernel<FMT_TF32>), nullptr, nullptr}, {ADN_K(pl_gemm_ms_kernel<FMT_F16>), nullptr, nullptr}}},
+    // Kernel::THIN: 64 x 64 units
+    {BN, true, 64, THIN_THREADS, THIN_SMEM_BYTES,
+     {{nullptr, nullptr, nullptr}, {ADN_K(pl_thin_kernel<EPI_BIAS_ACT>), ADN_K(pl_thin_kernel<EPI_MASK>), nullptr}}},
+    // Kernel::DW
+    {DW_BN, false, 0, DW_THREADS, DW_SMEM_BYTES, {{nullptr, nullptr, nullptr}, {nullptr, nullptr, ADN_K(pl_dw_kernel)}}},
+    // Kernel::WIDE: 64 x 64 units
+    {DW_BN, false, 64, DW_THREADS, WIDE_SMEM_BYTES,
+     {{nullptr, nullptr, nullptr}, {ADN_K(pl_wide_kernel<EPI_BIAS_ACT>), ADN_K(pl_wide_kernel<EPI_MASK>), nullptr}}},
+};
+#undef ADN_K
+static_assert(sizeof(kSpecs) / sizeof(kSpecs[0]) == (size_t)Kernel::WIDE + 1, "one KernelSpec per Kernel");
+static_assert(FMT_TF32 == 0 && FMT_F16 == 1 && EPI_BIAS_ACT == 0 && EPI_MASK == 1 && EPI_PARTIAL == 2, "KernelSpec::fn");
+
 __device__ unsigned int g_plane_overflow = 0u;
 
 static PFN_cuTensorMapEncodeTiled g_encode = nullptr;
@@ -1502,21 +1550,13 @@ int init() {
     }
     g_encode = reinterpret_cast<PFN_cuTensorMapEncodeTiled>(fn);
     bool ok = true;
-#define ADN_PL_ATTR(F, E) \
-  ok = ok && (cudaFuncSetAttribute(pl_gemm_kernel<F, E>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) == cudaSuccess)
-    ADN_PL_ATTR(FMT_TF32, EPI_BIAS_ACT); ADN_PL_ATTR(FMT_TF32, EPI_MASK); ADN_PL_ATTR(FMT_TF32, EPI_PARTIAL);
-    ADN_PL_ATTR(FMT_F16, EPI_BIAS_ACT); ADN_PL_ATTR(FMT_F16, EPI_MASK); ADN_PL_ATTR(FMT_F16, EPI_PARTIAL);
-#undef ADN_PL_ATTR
-    ok = ok && cudaFuncSetAttribute(pl_gemm_ms_kernel<FMT_TF32>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) == cudaSuccess;
-    ok = ok && cudaFuncSetAttribute(pl_gemm_ms_kernel<FMT_F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) == cudaSuccess;
-    ok = ok && cudaFuncSetAttribute(pl_thin_kernel<EPI_BIAS_ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, THIN_SMEM_BYTES) == cudaSuccess;
-    ok = ok && cudaFuncSetAttribute(pl_thin_kernel<EPI_MASK>, cudaFuncAttributeMaxDynamicSharedMemorySize, THIN_SMEM_BYTES) == cudaSuccess;
-    ok = ok && cudaFuncSetAttribute(pl_dw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DW_SMEM_BYTES) == cudaSuccess;
-    ok = ok && cudaFuncSetAttribute(pl_wide_kernel<EPI_BIAS_ACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, WIDE_SMEM_BYTES) == cudaSuccess;
-    ok = ok && cudaFuncSetAttribute(pl_wide_kernel<EPI_MASK>, cudaFuncAttributeMaxDynamicSharedMemorySize, WIDE_SMEM_BYTES) == cudaSuccess;
+    for (const KernelSpec& k : kSpecs)
+      for (const auto& per_fmt : k.fn)
+        for (const void* entry : per_fmt)
+          ok = ok && (!entry || cudaFuncSetAttribute(entry, cudaFuncAttributeMaxDynamicSharedMemorySize, k.smem) == cudaSuccess);
     if (!ok) {
       (void)cudaGetLastError();
-      rc = fail(ADN_ERR_CUDA, "pl::init: cudaFuncSetAttribute(smem=%d) failed", SMEM_BYTES);
+      rc = fail(ADN_ERR_CUDA, "pl::init: cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed");
       return;
     }
     void* addr = nullptr;
@@ -1604,7 +1644,7 @@ static int make_map(int fmt, CUtensorMap* map, const void* plane, int64_t rows, 
 
 // output planes (fp16) as TMA store targets: [box columns][box rows] boxes; box = 32 (pl_gemm_kernel's 32 x 32 slices,
 // 64 B rows, SWIZZLE_64B in shared memory) or 64 (pl_thin_kernel's and pl_wide_kernel's 64 x 64 units, 128 B rows, SWIZZLE_128B)
-static int make_store_map(CUtensorMap* map, const void* plane, int64_t rows, int64_t nkb, int box_rc = 32) {
+static int make_store_map(CUtensorMap* map, const void* plane, int64_t rows, int64_t nkb, int box_rc) {
   if (!g_encode) return fail(ADN_ERR_CUDA, "pl: adn_init() was not called");
   const MapKey key{plane, rows, nkb, 2, FMT_F16, box_rc};      // mn = 2: a store box
   {
@@ -1642,7 +1682,7 @@ struct GemmDesc {
 
 // bn: the B tile extent (columns of the result)
 static int encode_maps(int fmt, const GemmDesc& d, CUtensorMap* a_hi, CUtensorMap* a_lo, CUtensorMap* b_hi, CUtensorMap* b_lo,
-                       const char* what, int bn = BN) {
+                       const char* what, int bn) {
   if (!planes_aligned(d.a.hi) || !planes_aligned(d.a.lo) || !planes_aligned(d.b.hi) || !planes_aligned(d.b.lo))
     return fail(ADN_ERR_INVALID, "%s: plane buffers must be 256 B aligned", what);
   int rc;
@@ -1653,26 +1693,23 @@ static int encode_maps(int fmt, const GemmDesc& d, CUtensorMap* a_hi, CUtensorMa
   return ADN_OK;
 }
 
-// A group runs on pl_thin_kernel when every problem is one fp16 accumulation chunk with planes out and no split.
-static bool thin_group(int fmt, const Group& grp) {
-  if (fmt != FMT_F16) return false;
-  for (int i = 0; i < grp.n; ++i) {
-    const GemmParams& g = grp.p[i].g;
+// A group is thin-K when every problem is one fp16 accumulation chunk with planes out and no split.
+static bool thin_group(const GemmDesc* d, int m) {
+  for (int i = 0; i < m; ++i) {
+    const GemmParams& g = d[i].g;
     if (!g.out_planes || g.splits != 1 || g.total_kb > Fmt<FMT_F16>::CHUNK) return false;
   }
   return true;
 }
-// A dW group (EPI_PARTIAL) runs on pl_dw_kernel when the format is fp16, padding every problem's N to 128 columns
-// instead of 64 adds at most 1/8 to the group's MMA work, and the wide items still spread over the SMs: work items are
-// dealt round-robin and a wide item is two narrow items of work, so the busiest SM may get at most one narrow item's
-// work more than with 128 x 64 tiles.  (The split plan is made for 128 x 64 tiles: the first-layer dW of the
-// benchmarked step has 135 wide items for 132 SMs, and three SMs doing two of them made that wave 37 % slower.)
-// Reads M, N, total_kb and splits only, which the tile does not change.
-static bool dw_group(int fmt, const Group& grp) {
-  if (fmt != FMT_F16) return false;
+// A dW group qualifies for 128-column tiles when padding every problem's N to 128 columns instead of 64 adds at most
+// 1/8 to the group's MMA work, and the wide items still spread over the SMs: work items are dealt round-robin and a
+// wide item is two narrow items of work, so the busiest SM may get at most one narrow item's work more than with
+// 128 x 64 tiles.  (The split plan is made for 128 x 64 tiles: the first-layer dW of the benchmarked step has 135 wide
+// items for 132 SMs, and three SMs doing two of them made that wave 37 % slower.)
+static bool dw_group(const GemmDesc* d, int m) {
   int64_t narrow = 0, wide = 0, items_n = 0, items_w = 0;
-  for (int i = 0; i < grp.n; ++i) {
-    const GemmParams& g = grp.p[i].g;
+  for (int i = 0; i < m; ++i) {
+    const GemmParams& g = d[i].g;
     const int64_t tm = ceil_div(g.M, BM);
     narrow += tm * g.total_kb * ceil_div(g.N, BN) * BN;
     wide += tm * g.total_kb * ceil_div(g.N, DW_BN) * DW_BN;
@@ -1684,15 +1721,15 @@ static bool dw_group(int fmt, const Group& grp) {
 }
 // MMA work (k-blocks x tile columns) of the busiest CTA when the group's work items are dealt round-robin, tiles of
 // `bn` columns.  Problem i's items are a contiguous run, so CTA c gets full or full + 1 of them: O(problems x SMs).
-static int64_t busiest_cta_work(const Group& grp, int bn) {
+static int64_t busiest_cta_work(const GemmDesc* d, int m, int bn) {
   int64_t items = 0;
-  for (int i = 0; i < grp.n; ++i) items += ceil_div(grp.p[i].g.M, BM) * ceil_div(grp.p[i].g.N, bn) * grp.p[i].g.splits;
+  for (int i = 0; i < m; ++i) items += ceil_div(d[i].g.M, BM) * ceil_div(d[i].g.N, bn) * d[i].g.splits;
   const int64_t ctas = std::min<int64_t>(items, sm_count());
   if (ctas <= 0) return 0;
   std::vector<int64_t> work((size_t)ctas, 0);
   int64_t j0 = 0;
-  for (int i = 0; i < grp.n; ++i) {
-    const GemmParams& g = grp.p[i].g;
+  for (int i = 0; i < m; ++i) {
+    const GemmParams& g = d[i].g;
     const int64_t cnt = ceil_div(g.M, BM) * ceil_div(g.N, bn) * g.splits, w = (int64_t)g.kb_per_split * bn;
     const int64_t full = cnt / ctas, rem = cnt % ctas, first = j0 % ctas;
     for (int64_t c = 0; c < ctas; ++c) work[(size_t)c] += w * (full + ((c - first + ctas) % ctas < rem ? 1 : 0));
@@ -1700,138 +1737,119 @@ static int64_t busiest_cta_work(const Group& grp, int bn) {
   }
   return *std::max_element(work.begin(), work.end());
 }
-// A single-source forward or dX group runs on pl_wide_kernel when the format is fp16, every problem has planes out,
-// the group is not a thin-K group (pl_thin_kernel keeps those), padding every problem's N to 128 columns adds at most
-// 1/8 to the group's MMA work, and so does the wide tile to the busiest CTA's.  The second bound counts work, not
-// rounds as dw_group does: the layer waves mix problems of 1 to 16 k-blocks per item.  (The hidden-layer waves of the
-// benchmarked step deal 6,912 wide items in 53 rounds against 13,312 narrow ones in 101, which dw_group's rule
-// refuses, but the busiest CTA gets 1,052 k-blocks of 64 columns against 1,038.)  Dense fp32 outputs (the logits
-// forward, the conv stem's dX) and TF32 planes stay on pl_gemm_kernel.
-static bool wide_group(int fmt, const Group& grp) {
-  if (fmt != FMT_F16 || thin_group(fmt, grp)) return false;
+// A forward or dX group qualifies for 128-column tiles when every problem has planes out, padding every problem's N
+// to 128 columns adds at most 1/8 to the group's MMA work, and so does the wide tile to the busiest CTA's.  The second
+// bound counts work, not rounds as dw_group does: the layer waves mix problems of 1 to 16 k-blocks per item.  (The
+// hidden-layer waves of the benchmarked step deal 6,912 wide items in 53 rounds against 13,312 narrow ones in 101,
+// which dw_group's rule refuses, but the busiest CTA gets 1,052 k-blocks of 64 columns against 1,038.)  Dense fp32
+// outputs (the logits forward, the conv stem's dX) stay on pl_gemm_kernel.
+static bool wide_group(const GemmDesc* d, int m) {
   int64_t narrow = 0, wide = 0;
-  for (int i = 0; i < grp.n; ++i) {
-    const GemmParams& g = grp.p[i].g;
+  for (int i = 0; i < m; ++i) {
+    const GemmParams& g = d[i].g;
     if (!g.out_planes) return false;
     narrow += ceil_div(g.M, BM) * g.total_kb * ceil_div(g.N, BN) * BN;
     wide += ceil_div(g.M, BM) * g.total_kb * ceil_div(g.N, DW_BN) * DW_BN;
   }
-  return 8 * wide <= 9 * narrow && 8 * busiest_cta_work(grp, DW_BN) <= 9 * busiest_cta_work(grp, BN);
+  return 8 * wide <= 9 * narrow && 8 * busiest_cta_work(d, m, DW_BN) <= 9 * busiest_cta_work(d, m, BN);
 }
-template <int FMT, int EPI>
-static void launch_kernel(const Group& grp, int grid, cudaStream_t st) {
-  pl_gemm_kernel<FMT, EPI><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(grp);
+// The kernel for the m GEMMs d[0..m) of epilogue kind epi.  Multi-source forwards and TF32 planes run the general
+// kernels; an fp16 thin-K group (planes out, so never dW) runs pl_thin_kernel, a dW group pl_dw_kernel and a forward or
+// dX group pl_wide_kernel when their rules above hold; every other group runs pl_gemm_kernel.
+static Kernel choose_kernel(int fmt, int epi, bool multi_source, const GemmDesc* d, int m) {
+  if (multi_source) return Kernel::GEMM_MS;
+  if (fmt != FMT_F16) return Kernel::GEMM;
+  if (epi == EPI_PARTIAL) return dw_group(d, m) ? Kernel::DW : Kernel::GEMM;
+  if (thin_group(d, m)) return Kernel::THIN;
+  return wide_group(d, m) ? Kernel::WIDE : Kernel::GEMM;
 }
+
+// one persistent launch: a parameter block and the kernel that runs it
+template <class G>
+struct Launch {
+  Kernel kernel;
+  G grp;
+};
 // n independent GEMMs of the same epilogue kind -> parameter blocks of up to MAX_GROUP problems each, one per
-// persistent launch (G = MsGroup: multi-source forward GEMMs, on pl_gemm_ms_kernel).  Every descriptor is encoded
-// here, before anything is launched, so that a failure leaves every output as it was.
+// persistent launch (G = MsGroup: multi-source forward GEMMs).  Every descriptor is encoded here, before anything is
+// launched, so that a failure leaves every output as it was.
 template <int EPI, class G>
-static int build_groups(int fmt, const GemmDesc* d, int n, std::vector<G>& out, const char* what) {
+static int build_groups(int fmt, const GemmDesc* d, int n, std::vector<Launch<G>>& out, const char* what) {
   constexpr bool MS = std::is_same<G, MsGroup>::value;
   static_assert(!MS || EPI == EPI_BIAS_ACT, "multi-source GEMMs are forward only");
   out.clear();
-  {
-    for (int i0 = 0; i0 < n; i0 += MAX_GROUP) {
-      const int m = std::min(MAX_GROUP, n - i0);
-      out.emplace_back();
-      G& grp = out.back();
-      memset(&grp, 0, sizeof(grp));
-      // the tile width: 128 columns when the group goes to pl_dw_kernel or pl_wide_kernel (dw_group and wide_group
-      // read only the parameters set here)
-      int bn = BN;
-      if constexpr (!MS) {
-        for (int i = 0; i < m; ++i) grp.p[i].g = d[i0 + i].g;
-        grp.n = m;
-        if (EPI == EPI_PARTIAL ? dw_group(fmt, grp) : wide_group(fmt, grp)) bn = DW_BN;
-      }
-      int items = 0;
-      for (int i = 0; i < m; ++i) {
-        const GemmDesc& src = d[i0 + i];
-        auto& pr = grp.p[i];
-        // the kernel fixes the operand majorness per epilogue kind (fwd: K / MN, dX: K / K, dW: MN / MN)
-        if (src.a.mn_major != (EPI == EPI_PARTIAL) || src.b.mn_major != (EPI != EPI_MASK))
-          return fail(ADN_ERR_INVALID, "%s: operand majorness does not match the epilogue kind", what);
-        int rc = encode_maps(fmt, src, &pr.a_hi, &pr.a_lo, &pr.b_hi, &pr.b_lo, what, bn);
-        if (rc) return rc;
-        if constexpr (MS) {
-          int kb = (int)src.a.nkb;
-          pr.n_src = src.n_src;
-          pr.kb_end[0] = kb;
-          for (int q = 0; q < src.n_src; ++q) {
-            GemmDesc piece;
-            piece.a = src.sa[q];
-            piece.b = src.sb[q];
-            if ((rc = encode_maps(fmt, piece, &pr.src[q][0], &pr.src[q][1], &pr.src[q][2], &pr.src[q][3], what))) return rc;
-            kb += (int)src.sa[q].nkb;
-            pr.kb_end[q + 1] = kb;
-          }
-          if (kb != src.g.total_kb) return fail(ADN_ERR_INVALID, "%s: k-blocks of the pieces do not add up", what);
+  for (int i0 = 0; i0 < n; i0 += MAX_GROUP) {
+    const int m = std::min(MAX_GROUP, n - i0);
+    out.emplace_back();
+    Launch<G>& l = out.back();
+    G& grp = l.grp;
+    memset(&grp, 0, sizeof(grp));
+    l.kernel = choose_kernel(fmt, EPI, MS, d + i0, m);
+    const KernelSpec& k = kSpecs[(int)l.kernel];
+    int items = 0;
+    for (int i = 0; i < m; ++i) {
+      const GemmDesc& src = d[i0 + i];
+      auto& pr = grp.p[i];
+      // the kernel fixes the operand majorness per epilogue kind (fwd: K / MN, dX: K / K, dW: MN / MN)
+      if (src.a.mn_major != (EPI == EPI_PARTIAL) || src.b.mn_major != (EPI != EPI_MASK))
+        return fail(ADN_ERR_INVALID, "%s: operand majorness does not match the epilogue kind", what);
+      int rc = encode_maps(fmt, src, &pr.a_hi, &pr.a_lo, &pr.b_hi, &pr.b_lo, what, k.tbn);
+      if (rc) return rc;
+      if constexpr (MS) {
+        int kb = (int)src.a.nkb;
+        pr.n_src = src.n_src;
+        pr.kb_end[0] = kb;
+        for (int q = 0; q < src.n_src; ++q) {
+          GemmDesc piece;
+          piece.a = src.sa[q];
+          piece.b = src.sb[q];
+          if ((rc = encode_maps(fmt, piece, &pr.src[q][0], &pr.src[q][1], &pr.src[q][2], &pr.src[q][3], what, k.tbn))) return rc;
+          kb += (int)src.sa[q].nkb;
+          pr.kb_end[q + 1] = kb;
         }
-        pr.g = src.g;
-        // fp16 plane tiles leave the epilogue by TMA stores (the API checked yp / dxp against planes_aligned):
-        // pl_gemm_kernel's 32 x 32 slices, or pl_wide_kernel's 64 x 64 units
-        if (fmt == FMT_F16 && src.g.out_planes) {
-          const int box = bn == DW_BN ? 64 : 32;
-          if ((rc = make_store_map(&pr.o_hi, src.g.out, src.g.M, src.g.out_nb32 / 2, box))) return rc;
-          if ((rc = make_store_map(&pr.o_lo, src.g.out_lo, src.g.M, src.g.out_nb32 / 2, box))) return rc;
-        }
-        pr.g.a_mn = src.a.mn_major;
-        pr.g.b_mn = src.b.mn_major;
-        pr.g.tiles_m = (int)ceil_div(pr.g.M, BM);
-        pr.g.tiles_n = (int)ceil_div(pr.g.N, bn);
-        pr.g.tiles = pr.g.tiles_m * pr.g.tiles_n;
-        if ((int64_t)pr.g.tiles * pr.g.splits >= (1 << 21))
-          return fail(ADN_ERR_UNSUPPORTED, "%s: %d work items exceed the decode range", what, pr.g.tiles * pr.g.splits);
-        pr.g.inv_tiles = 1.0f / (float)pr.g.tiles;
-        pr.g.inv_tiles_n = 1.0f / (float)pr.g.tiles_n;
-        pr.g.ovf = g_ovf_addr;
-        pr.item0 = items;
-        items += pr.g.tiles_m * pr.g.tiles_n * pr.g.splits;
+        if (kb != src.g.total_kb) return fail(ADN_ERR_INVALID, "%s: k-blocks of the pieces do not add up", what);
       }
-      grp.n = m;
-      grp.total_items = items;
-      if constexpr (!MS) {
-        if (thin_group(fmt, grp)) {     // pl_thin_kernel's work items (128-row block x run of THIN_RUN N tiles) and store boxes
-          items = 0;
-          for (int i = 0; i < m; ++i) {
-            Problem& pr = grp.p[i];
-            pr.item0 = items;
-            items += pr.g.tiles_m * thin_runs(pr.g.tiles_n);
-            int rc;
-            if ((rc = make_store_map(&pr.o_hi, pr.g.out, pr.g.M, pr.g.out_nb32 / 2, 64))) return rc;
-            if ((rc = make_store_map(&pr.o_lo, pr.g.out_lo, pr.g.M, pr.g.out_nb32 / 2, 64))) return rc;
-          }
-          grp.total_items = items;
-        }
+      pr.g = src.g;
+      // fp16 plane tiles leave the epilogue by TMA stores (the API checked yp / dxp against planes_aligned)
+      if (fmt == FMT_F16 && src.g.out_planes) {
+        if ((rc = make_store_map(&pr.o_hi, src.g.out, src.g.M, src.g.out_nb32 / 2, k.store_box))) return rc;
+        if ((rc = make_store_map(&pr.o_lo, src.g.out_lo, src.g.M, src.g.out_nb32 / 2, k.store_box))) return rc;
       }
+      pr.g.a_mn = src.a.mn_major;
+      pr.g.b_mn = src.b.mn_major;
+      pr.g.tiles_m = (int)ceil_div(pr.g.M, BM);
+      pr.g.tiles_n = (int)ceil_div(pr.g.N, k.tbn);
+      pr.g.tiles = pr.g.tiles_m * pr.g.tiles_n;
+      if ((int64_t)pr.g.tiles * pr.g.splits >= (1 << 21))
+        return fail(ADN_ERR_UNSUPPORTED, "%s: %d work items exceed the decode range", what, pr.g.tiles * pr.g.splits);
+      pr.g.inv_tiles = 1.0f / (float)pr.g.tiles;
+      pr.g.inv_tiles_n = 1.0f / (float)pr.g.tiles_n;
+      pr.g.ovf = g_ovf_addr;
+      pr.item0 = items;
+      items += pr.g.tiles_m * (k.row_runs ? thin_runs(pr.g.tiles_n) : pr.g.tiles_n * pr.g.splits);
     }
+    grp.n = m;
+    grp.total_items = items;
   }
   return ADN_OK;
 }
 template <int EPI, class G>
-static int launch_groups(int fmt, const std::vector<G>& groups, cudaStream_t st, const char* what) {
-  for (const G& grp : groups) {
-    const int grid = std::min(grp.total_items, sm_count());
-    if constexpr (std::is_same<G, MsGroup>::value) {
-      if (fmt == FMT_F16) pl_gemm_ms_kernel<FMT_F16><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(grp);
-      else pl_gemm_ms_kernel<FMT_TF32><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(grp);
-    } else if (thin_group(fmt, grp)) {
-      if constexpr (EPI != EPI_PARTIAL) pl_thin_kernel<EPI><<<grid, THIN_THREADS, THIN_SMEM_BYTES, st>>>(grp);
-    } else if (EPI == EPI_PARTIAL && dw_group(fmt, grp)) {
-      pl_dw_kernel<<<grid, DW_THREADS, DW_SMEM_BYTES, st>>>(grp);
-    } else if (EPI != EPI_PARTIAL && wide_group(fmt, grp)) {
-      if constexpr (EPI != EPI_PARTIAL) pl_wide_kernel<EPI><<<grid, DW_THREADS, WIDE_SMEM_BYTES, st>>>(grp);
-    } else {
-      if (fmt == FMT_F16) launch_kernel<FMT_F16, EPI>(grp, grid, st);
-      else launch_kernel<FMT_TF32, EPI>(grp, grid, st);
-    }
+static int launch_groups(int fmt, const std::vector<Launch<G>>& groups, cudaStream_t st, const char* what) {
+  for (const Launch<G>& l : groups) {
+    const KernelSpec& k = kSpecs[(int)l.kernel];
+    const void* entry = k.fn[fmt][EPI];
+    if (!entry)      // choose_kernel returns only kinds with an entry point for the format and epilogue kind
+      return fail(ADN_ERR_UNSUPPORTED, "%s: kernel kind %d has no entry point for format %d, epilogue %d", what, (int)l.kernel,
+                  fmt, EPI);
+    void* args[] = {const_cast<G*>(&l.grp)};
+    (void)cudaLaunchKernel(entry, std::min(l.grp.total_items, sm_count()), k.threads, args, k.smem, st);
     ADN_CHECK_LAUNCH(what);
   }
   return ADN_OK;
 }
 template <int EPI>
 static int launch_group(int fmt, const GemmDesc* d, int n, cudaStream_t st, const char* what) {
-  std::vector<Group> groups;
+  std::vector<Launch<Group>> groups;
   const int rc = build_groups<EPI>(fmt, d, n, groups, what);
   return rc ? rc : launch_groups<EPI>(fmt, groups, st, what);
 }
@@ -1922,8 +1940,8 @@ int dense_fwd_group(int fmt, const FwdOp* ops, int n, int64_t batch, cudaStream_
     (o.n_srcs ? dm : d).push_back(e);
   }
   // both kinds are encoded before either is launched: a call that returns an error has written nothing
-  std::vector<Group> groups;
-  std::vector<MsGroup> ms_groups;
+  std::vector<Launch<Group>> groups;
+  std::vector<Launch<MsGroup>> ms_groups;
   int rc;
   if ((rc = build_groups<EPI_BIAS_ACT>(fmt, d.data(), (int)d.size(), groups, "pl dense_fwd gemm"))) return rc;
   if ((rc = build_groups<EPI_BIAS_ACT>(fmt, dm.data(), (int)dm.size(), ms_groups, "pl dense_fwd multi-source gemm"))) return rc;

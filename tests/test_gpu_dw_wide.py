@@ -9,17 +9,12 @@ cap of 64 splits and the same 40,960 entries, so both calls run the op on the sa
 number of partial sums each call wrote back from the op's workspace to show that, then requires dW to agree byte for
 byte.  Every result is also checked against float64 with the componentwise bounds of test_gpu_plane_groups.
 
-The kernel-choice checks read kernel names from torch.profiler.  They run in a child process: profiling a whole
-training step here left later profiler sessions of the same process without CUDA events.
+The kernel-choice checks read kernel names from torch.profiler in a child process (tests/plane_kernels.py).
 """
-
-import json
-import os
-import subprocess
-import sys
 
 import pytest
 
+from tests.plane_kernels import in_child, kernels as _kernels
 from tests.test_gpu_plane_groups import _bwd_bufs, _bwd_call, _bwd_case, _bwd_check, _bwd_struct, _bytes_equal, _open
 
 pytestmark = pytest.mark.gpu
@@ -101,17 +96,6 @@ def test_dw_wide_matches_general(env, B):
     assert max(split_counts) > 1, split_counts
 
 
-def _kernels(torch, fn):
-  """names of the plane GEMM kernels fn launches, in order"""
-  from torch.profiler import ProfilerActivity, profile
-  torch.cuda.synchronize()
-  with profile(activities=[ProfilerActivity.CUDA]) as prof:
-    fn()
-    torch.cuda.synchronize()
-  return [e.name for e in prof.events()
-          if e.device_type.name == "CUDA" and any(k in e.name for k in ("pl_dw_kernel", "pl_gemm_kernel", "pl_thin_kernel"))]
-
-
 def _choice_groups():
   """kernel names of single dW group calls, fp16 and TF32: [(label, names)]"""
   torch, _lib, lib = _open()
@@ -129,41 +113,6 @@ def _choice_groups():
   return out
 
 
-def _choice_step():
-  """kernel names of one eager training step of bench.py's workload (8 candidates 100 -> H -> H -> 10, B = 32768)"""
-  torch, _lib, lib = _open()
-  import bench
-  from adanet_b200.core import engine as eng
-  from adanet_b200.core import search as srch
-  dev = torch.device("cuda", 0)
-  x_np, y_np = bench.make_tabular(2 * bench.BATCH, bench.IN_DIM, bench.CLASSES, seed=1234)
-  x_dev, y_dev = torch.as_tensor(x_np).to(dev), torch.as_tensor(y_np).to(dev)
-  ens = eng.EnsemblerPlanSpec(optimizer=("sgd", bench.ENS_LR), adanet_lambda=bench.LAMBDA, adanet_beta=bench.BETA)
-  space = lambda t, frozen: [eng.SubnetworkPlanSpec(n, d, cx, ("sgd", bench.SUB_LR), ws, bs, shared={"num_layers": 2})
-                             for n, d, cx, ws, bs in bench.candidate_weights(t)]
-  s = srch.AdaNetSearch(space, ens, bench.IN_DIM, bench.CLASSES, bench.BATCH, device=dev, keep_traces=False,
-                        placement="balanced")
-  plan = s.build_iteration()
-  plan.use_cuda_graph = False
-  batches = srch.consecutive_batches(x_dev, y_dev, bench.BATCH)
-  plan.train_step(*next(batches))
-  return _kernels(torch, lambda: plan.train_step(*next(batches)))
-
-
-def _in_child(what):
-  """runs _choice_<what>() in a fresh interpreter started like this one and returns its result"""
-  root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-  flags = [f for f, on in (("-I", sys.flags.isolated), ("-E", sys.flags.ignore_environment),
-                           ("-s", sys.flags.no_user_site)) if on]
-  code = ("import json, sys; sys.path.insert(0, %r); from tests import test_gpu_dw_wide as t; "
-          "print('RESULT ' + json.dumps(t._choice_%s()))" % (root, what))
-  r = subprocess.run([sys.executable] + flags + ["-c", code], cwd=root, capture_output=True, text=True, timeout=900)
-  lines = [l for l in r.stdout.splitlines() if l.startswith("RESULT ")]
-  assert r.returncode == 0 and lines, "child process failed (%d):\n%s\n%s" % (r.returncode, r.stdout[-3000:],
-                                                                         r.stderr[-3000:])
-  return json.loads(lines[-1][len("RESULT "):])
-
-
 def test_kernel_choice(env):
   want = {"200x65": "pl_dw_kernel",                 # padding 65 columns to 128 costs nothing
           "100x64": "pl_gemm_kernel<1, 2>",         # padding 64 columns to 128 doubles the work
@@ -171,7 +120,7 @@ def test_kernel_choice(env):
           "100x64+narrow": "pl_gemm_kernel<1, 2>",
           "1024x1024+narrow": "pl_gemm_kernel<1, 2>",
           "tf32": "pl_gemm_kernel<0, 2>"}
-  got = _in_child("groups")
+  got = in_child("test_gpu_dw_wide", "_choice_groups")
   assert [label for label, _ in got] == list(want), got
   for label, names in got:
     assert len(names) == 1 and want[label] in names[0], (label, names)
@@ -181,7 +130,7 @@ def test_bench_step_kernel_choice(env):
   """The benchmarked training step (bench.py's 8 candidates 100 -> H -> H -> 10): its hidden-layer dW launch runs
   pl_dw_kernel.  The logits-layer dW (N = 10) runs pl_gemm_kernel<fp16, EPI_PARTIAL>, and so does the first-layer dW,
   whose 135 wide work items would leave three SMs with two each."""
-  names = _in_child("step")
+  names = in_child("plane_kernels", "bench_step_kernels")
   dw = [n for n in names if "pl_dw_kernel" in n or "pl_gemm_kernel<1, 2>" in n]
   # the backward visits the logits layer first, then the hidden layer, then the first layer
   assert len(dw) == 3, names

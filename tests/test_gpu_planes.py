@@ -266,6 +266,27 @@ def test_tma_descriptor_cache(env):
   assert _lib.query(_lib.Q_TMA_MAP_CACHE_MISSES) == m0
   assert _lib.query(_lib.Q_TMA_MAP_CACHE_HITS) == h0 + 12
 
+  def lookups(B, I, O, planes_out):
+    """descriptor lookups (hits + misses) of one forward call"""
+    xq = _planes(torch, _lib, lib, rng.standard_normal((B, I)).astype(np.float32))
+    wq = _planes(torch, _lib, lib, rng.standard_normal((I, O)).astype(np.float32))
+    out = (torch.empty((_lib.query(_lib.Q_PLANES_BYTES, B, O) // 4,), device="cuda") if planes_out
+           else torch.empty((B, O), device="cuda"))
+    yp, yd = (out.data_ptr(), None) if planes_out else (None, out.data_ptr())
+    n0 = _lib.query(_lib.Q_TMA_MAP_CACHE_HITS) + _lib.query(_lib.Q_TMA_MAP_CACHE_MISSES)
+    _lib.check(lib.adn_dense_fwd_p(xq.data_ptr(), wq.data_ptr(), None, yp, yd, B, I, O, 0, sp), "fwd_p")
+    return _lib.query(_lib.Q_TMA_MAP_CACHE_HITS) + _lib.query(_lib.Q_TMA_MAP_CACHE_MISSES) - n0
+
+  # every kernel looks up the descriptors it reads and no others: A and B hi / lo', and with fp16 planes out the
+  # hi / lo' store boxes (TF32 planes store rows directly).  The counts do not tell the kernels apart; the comments
+  # name the fp16 kernel each shape runs on, which the kernel-choice tests check.
+  stores = 2 if _lib.plane_format() == _lib.PLANES_F16 else 0
+  assert lookups(256, 96, 80, False) == 4                 # dense out: pl_gemm_kernel
+  assert lookups(256, 96, 80, True) == 4 + stores         # K <= 128: pl_thin_kernel
+  assert lookups(8192, 256, 1024, True) == 4 + stores     # N = 1024 on 64 row blocks: pl_wide_kernel
+  assert lookups(256, 256, 80, True) == 4 + stores        # 2 wide items against 4 narrow ones would double the
+                                                          # busiest CTA's work: pl_gemm_kernel
+
 
 
 

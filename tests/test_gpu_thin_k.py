@@ -9,6 +9,7 @@ results must agree byte for byte -- hi and lo' planes, sign-bit words, the per-3
 import numpy as np
 import pytest
 
+from tests.plane_kernels import kernels as _kernels
 from tests.test_gpu_plane_groups import (DX_MUL, _bwd_case, _bwd_check, _bwd_run, _bytes_equal, _fwd_case, _fwd_check,
                                          _fwd_run, _fwd_struct, _open, _stream)
 
@@ -112,16 +113,6 @@ def test_dx_thin_matches_general(env, B):
       fails.append("op %d: per-32-row column sums differ between the kernels" % k)
   assert not _lib.plane_overflow()
   assert not fails, "\n".join(fails)
-
-
-def _kernels(torch, fn):
-  """names of the plane GEMM kernels fn launches, in order"""
-  from torch.profiler import ProfilerActivity, profile
-  torch.cuda.synchronize()
-  with profile(activities=[ProfilerActivity.CUDA]) as prof:
-    fn()
-    torch.cuda.synchronize()
-  return [e.name for e in prof.events() if "pl_thin_kernel" in e.name or "pl_gemm_kernel" in e.name]
 
 
 def test_kernel_choice(env):

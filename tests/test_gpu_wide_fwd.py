@@ -9,16 +9,12 @@ sums and their reduction -- and each is checked against float64 with the compone
 test_gpu_plane_groups.  N is not a multiple of 128 in most ops, so the second 64-column unit of the last tile lies
 partly or wholly past the output.
 
-The kernel-choice checks read kernel names from torch.profiler in a child process, as test_gpu_dw_wide does.
+The kernel-choice checks read kernel names from torch.profiler in a child process (tests/plane_kernels.py).
 """
-
-import json
-import os
-import subprocess
-import sys
 
 import pytest
 
+from tests.plane_kernels import in_child, kernels as _kernels
 from tests.test_gpu_plane_groups import (DX_MUL, _bwd_case, _bwd_check, _bwd_run, _bytes_equal, _fwd_case, _fwd_check,
                                          _fwd_run, _fwd_struct, _open, _stream)
 from tests.test_gpu_thin_k import _colsum_part
@@ -127,31 +123,6 @@ def test_dx_wide_matches_general(env, B):
   assert not fails, "\n".join(fails)
 
 
-KERNELS = ("pl_wide_kernel", "pl_gemm_kernel", "pl_thin_kernel", "pl_gemm_ms_kernel")
-
-
-def _kernels(torch, fn):
-  """short names (pl_wide_kernel<0>, pl_gemm_kernel<1, 0>, ...) of the plane GEMM kernels fn launches, in order"""
-  from torch.profiler import ProfilerActivity, profile
-  torch.cuda.synchronize()
-  with profile(activities=[ProfilerActivity.CUDA]) as prof:
-    fn()
-    torch.cuda.synchronize()
-  out = []
-  for e in prof.events():
-    if e.device_type.name != "CUDA":
-      continue
-    if "pl_dw_kernel" in e.name:
-      out.append("pl_dw_kernel")
-      continue
-    for k in KERNELS:
-      i = e.name.find(k + "<")
-      if i >= 0:
-        out.append(e.name[i:].split(">")[0] + ">")
-        break
-  return out
-
-
 def _choice_groups():
   """kernel names of single forward / dX group calls: [(label, names)]"""
   torch, _lib, lib = _open()
@@ -187,41 +158,6 @@ def _choice_groups():
   return out
 
 
-def _choice_step():
-  """kernel names of one eager training step of bench.py's workload (8 candidates 100 -> H -> H -> 10, B = 32768)"""
-  torch, _, _ = _open()
-  import bench
-  from adanet_b200.core import engine as eng
-  from adanet_b200.core import search as srch
-  dev = torch.device("cuda", 0)
-  x_np, y_np = bench.make_tabular(2 * bench.BATCH, bench.IN_DIM, bench.CLASSES, seed=1234)
-  x_dev, y_dev = torch.as_tensor(x_np).to(dev), torch.as_tensor(y_np).to(dev)
-  ens = eng.EnsemblerPlanSpec(optimizer=("sgd", bench.ENS_LR), adanet_lambda=bench.LAMBDA, adanet_beta=bench.BETA)
-  space = lambda t, frozen: [eng.SubnetworkPlanSpec(n, d, cx, ("sgd", bench.SUB_LR), ws, bs, shared={"num_layers": 2})
-                             for n, d, cx, ws, bs in bench.candidate_weights(t)]
-  s = srch.AdaNetSearch(space, ens, bench.IN_DIM, bench.CLASSES, bench.BATCH, device=dev, keep_traces=False,
-                        placement="balanced")
-  plan = s.build_iteration()
-  plan.use_cuda_graph = False
-  batches = srch.consecutive_batches(x_dev, y_dev, bench.BATCH)
-  plan.train_step(*next(batches))
-  return _kernels(torch, lambda: plan.train_step(*next(batches)))
-
-
-def _in_child(what):
-  """runs _choice_<what>() in a fresh interpreter started like this one and returns its result"""
-  root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-  flags = [f for f, on in (("-I", sys.flags.isolated), ("-E", sys.flags.ignore_environment),
-                           ("-s", sys.flags.no_user_site)) if on]
-  code = ("import json, sys; sys.path.insert(0, %r); from tests import test_gpu_wide_fwd as t; "
-          "print('RESULT ' + json.dumps(t._choice_%s()))" % (root, what))
-  r = subprocess.run([sys.executable] + flags + ["-c", code], cwd=root, capture_output=True, text=True, timeout=900)
-  lines = [l for l in r.stdout.splitlines() if l.startswith("RESULT ")]
-  assert r.returncode == 0 and lines, "child process failed (%d):\n%s\n%s" % (r.returncode, r.stdout[-3000:],
-                                                                         r.stderr[-3000:])
-  return json.loads(lines[-1][len("RESULT "):])
-
-
 def test_kernel_choice(env):
   # 64 x 4 ... 13 k-blocks on 2 row blocks: too few items to fill the SMs twice over, so wide tiles would leave the
   # busiest CTA twice the work
@@ -238,7 +174,7 @@ def test_kernel_choice(env):
     for kind, epi, ops in (("fwd", 0, FWD_OPS), ("dx", 1, BWD_OPS)):
       for call in _ops(Bw, ops)[1]:
         want["%s B=%d %s" % (kind, Bw, call)] = ["pl_wide_kernel<%d>" % epi]
-  got = _in_child("groups")
+  got = in_child("test_gpu_wide_fwd", "_choice_groups")
   assert [label for label, _ in got] == list(want), got
   for label, names in got:
     assert names == want[label], (label, names)
@@ -248,7 +184,7 @@ def test_bench_step_kernel_choice(env):
   """The benchmarked training step (bench.py's 8 candidates 100 -> H -> H -> 10): its hidden-layer forward and dX
   launches run pl_wide_kernel; the first-layer forward (K = 100) and the logits layer's dX (K = 10) stay on
   pl_thin_kernel, and no dX runs on pl_gemm_kernel."""
-  seq = _in_child("step")
+  seq = in_child("plane_kernels", "bench_step_kernels")
   for k in ("pl_wide_kernel<0>", "pl_wide_kernel<1>", "pl_thin_kernel<0>", "pl_thin_kernel<1>"):
     assert seq.count(k) == 1, seq
   assert "pl_gemm_kernel<1, 1>" not in seq, seq
